@@ -39,9 +39,10 @@
 //             warps 4-7 commit, when the batch has at most 16 tasks).
 //
 // The job at which a batch stops (its pick failed the exact test, so the walk
-// has to continue past it), jobs wider than a batch and tiny partitions take
-// the ONE-JOB PATH: the same walk in chunks of 32 candidates, every candidate
-// tested exactly, the first node_num passing ones taken.
+// has to continue past it), jobs wider than a batch, jobs with a general task
+// distribution and tiny partitions take the ONE-JOB PATH (single2): the same
+// walk in windows of 256 order positions, up to 32 candidates of a window tested
+// exactly at once, the first node_num passing ones taken.
 //
 // Why the result equals the sequential loop: a job's pick is "the first K nodes
 // in the order that pass". Candidates of the batch-start state are a superset
@@ -61,14 +62,11 @@ constexpr int kMaxJ = 32;          // jobs per batch
 constexpr int kMaxT = kNG;         // (job, node) tasks per batch: one group each
 constexpr int kBlk = 32;           // order positions per bounds block
 constexpr int kRingMax = 64;       // prefetch ring depth (jobs)
-constexpr int kValidateFor = 8;     // batches with up-front validation after a pick failed the exact test
-constexpr int kSpare = 12;          // ... during which every job lists this many candidates more than it needs
-constexpr int kRK = 64;             // nodes re-keyed at once (more: full sort)
+constexpr int kValidateFor = 8;    // batches with up-front validation after a pick failed the exact test
+constexpr int kSpare = 12;         // ... during which every job lists this many candidates more than it needs
+constexpr int kRK = 64;            // nodes re-keyed by one event-based rebuild (more: full sort)
 constexpr int kHeapMax = 128;      // general task distribution: top-K heaps of up to 127 nodes
-constexpr int kDeltaClasses = 4;
-#ifndef CRANE_SPEC_EVAL
-#define CRANE_SPEC_EVAL 1          // warps 1-7 test each slot's first guess while warp 0 resolves (A/B on config 2:
-#endif                             // 961k vs 918k decisions/s with the speculation off)   // res_total classes with a pre-computed cost delta per batch job            // nodes re-keyed by one event-based rebuild
+constexpr int kDeltaClasses = 4;   // res_total classes with a pre-computed cost delta per batch job
 static_assert(kMaxT <= 32 && kMaxJ <= 32, "resolve lays a batch over one warp's ballots");
 
 struct Smem2 {
@@ -131,18 +129,24 @@ __device__ __forceinline__ uint64_t g_and64(uint64_t v) {
 // ---- a node's timeline worked on by one group ------------------------------------
 struct Win2 {            // window minimum of one node (JobScheduler.cpp:5314-5319)
   uint64_t c0, c1, c2, c3, g0, g1;
+  int64_t cpu;           // cpu/mem/mem_sw minima (g_window<true> only)
+  uint64_t mem, mem_sw;
   bool ok;               // cpu/mem (or, exclusive: res_total) hold in every segment of the window
 };
 
 // Segments that start before w_end: cpu/mem tested per segment, core and gres
 // masks AND-reduced ("the window minimum", algebra.cuh). Exclusive jobs: every
-// segment must still hold res_total (JobScheduler.cpp:5285-5293). Two entries
-// per lane and round, so the loads of 16 entries are in flight together.
+// segment must still hold res_total (JobScheduler.cpp:5285-5293). kMinima: the
+// cpu/mem/mem_sw minima over the window too (general task distribution, which
+// counts tasks on the window minimum row itself).
+template <bool kMinima = false>
 __device__ __forceinline__ void g_window(const TlEntry* E, uint32_t n, int64_t w_end, int64_t req_cpu, uint64_t req_mem,
                                          bool exclusive, bool with_gres, const Row& tot, bool act, Win2& w) {
   const uint32_t gl = g_lane();
   const uint64_t ones = ~0ull;
   uint64_t c0 = ones, c1 = ones, c2 = ones, c3 = ones, g0 = ones, g1 = ones;
+  int64_t mcpu = INT64_MAX;
+  uint64_t mmem = ones, msw = ones;
   bool ok = true, more = act;
   for (uint32_t base = 0; __any_sync(kFullMask, more); base += kGL) {
     const uint32_t i0 = base + gl;
@@ -152,6 +156,11 @@ __device__ __forceinline__ void g_window(const TlEntry* E, uint32_t n, int64_t w
     if (ld0) e0 = E[i0];
     const bool in0 = ld0 && e0.t < w_end;
     if (in0) {
+      if constexpr (kMinima) {
+        mcpu = e0.seg.cpu_raw < mcpu ? e0.seg.cpu_raw : mcpu;
+        mmem = e0.seg.mem < mmem ? e0.seg.mem : mmem;
+        msw = e0.seg.mem_sw < msw ? e0.seg.mem_sw : msw;
+      }
       if (exclusive) ok = ok && row_le(tot, e0.seg);
       else {
         ok = ok && e0.seg.cpu_raw >= req_cpu && e0.seg.mem >= req_mem;
@@ -169,6 +178,17 @@ __device__ __forceinline__ void g_window(const TlEntry* E, uint32_t n, int64_t w
     w.c0 = g_and64(c0); w.c1 = g_and64(c1); w.c2 = g_and64(c2); w.c3 = g_and64(c3);
     if (__any_sync(kFullMask, act && with_gres)) { w.g0 = g_and64(g0); w.g1 = g_and64(g1); }
   }
+  if constexpr (kMinima) {
+#pragma unroll
+    for (int o = 1; o < kGL; o <<= 1) {
+      const int64_t oc = shfl_i64(mcpu, lane_id() ^ o);
+      const uint64_t om = shfl_u64(mmem, lane_id() ^ o), os = shfl_u64(msw, lane_id() ^ o);
+      mcpu = oc < mcpu ? oc : mcpu;
+      mmem = om < mmem ? om : mmem;
+      msw = os < msw ? os : msw;
+    }
+    w.cpu = mcpu; w.mem = mmem; w.mem_sw = msw;
+  }
 }
 // the row GetFeasibleResourceInNode sees for an immediate start: res_avail
 // Ckmin'ed with the window (cpu/mem already verified segment by segment)
@@ -179,6 +199,14 @@ __device__ __forceinline__ void win_row(const Win2& w, const Row& a0, const View
   wr.core[0] = a0.core[0] & w.c0; wr.core[1] = a0.core[1] & w.c1;
   wr.core[2] = a0.core[2] & w.c2; wr.core[3] = a0.core[3] & w.c3;
   wr.g[0] = a0.g[0] & w.g0; wr.g[1] = a0.g[1] & w.g1;
+}
+// the same with cpu/mem/mem_sw Ckmin'ed as well (w from g_window<true>): the row
+// the general task distribution counts tasks on
+__device__ __forceinline__ void win_row_min(const Win2& w, const Row& a0, const View& req, Row& wr) {
+  win_row(w, a0, req, wr);
+  wr.cpu_raw = a0.cpu_raw < w.cpu ? a0.cpu_raw : w.cpu;
+  wr.mem = a0.mem < w.mem ? a0.mem : w.mem;
+  wr.mem_sw = a0.mem_sw < w.mem_sw ? a0.mem_sw : w.mem_sw;
 }
 
 // earliest t >= T0 such that `alloc` <= every segment overlapping [t, t+limit)
@@ -455,9 +483,9 @@ __device__ __forceinline__ void jsel_load(const JobQ& jq, const uint32_t* bits, 
   js.req_cpu = jq.req.cpu_raw;
   js.spec8 = jq.spec8;
   js.name_need = jq.name_need;
-  js.gnames = (jq.flags >> 8) & 0xffu;
-  js.exclusive = jq.flags & 1u;
-  js.has_gres = jq.flags & 2u;
+  js.gnames = jq_gnames(jq);
+  js.exclusive = jq_exclusive(jq);
+  js.has_gres = jq_has_gres(jq);
 }
 __device__ __forceinline__ bool capable2(const Smem2& sm, const JSel2& js, uint32_t q) {
   return ((js.bits[q >> 5] >> (q & 31)) & 1u) && !sm.skip[q];
@@ -545,7 +573,7 @@ __device__ __forceinline__ void select2(const Smem2& sm, uint32_t mp, const JSel
 // when the job is placed on it
 __device__ __forceinline__ double new_cost2(const JobQ& jq, uint32_t q, const double* cost) {
   const int64_t tot_cpu = node_total_cpu2(q);
-  return __dadd_rn(cost[q], cost_step(s2_cx.cost_policy, jq.time_limit, (jq.flags & 1u) ? tot_cpu : jq.req.cpu_raw, tot_cpu));
+  return __dadd_rn(cost[q], cost_step(s2_cx.cost_policy, jq.time_limit, jq_exclusive(jq) ? tot_cpu : jq.req.cpu_raw, tot_cpu));
 }
 
 // block-wide exclusive prefix over one value per thread (kT2 threads)
@@ -833,6 +861,60 @@ __device__ __forceinline__ void write_node2(const JobQ& jq, uint32_t q, uint32_t
   s2_cx.out.alloc_res[dst] = alloc;
   s2_cx.tl.n[s2_cx.base + q] = nn;
 }
+// output slot of a job's node q: its rank among the job's K nodes node(0..K) by node index
+// (deviation D3), by one group
+template <class NodeAt>
+__device__ __forceinline__ uint32_t g_out_rank(uint32_t K, uint32_t q, bool act, NodeAt node) {
+  uint32_t rank = 0;
+  if (act && K > 1)
+    for (uint32_t m = g_lane(); m < K; m += kGL) rank += node(m) < q ? 1u : 0u;
+#pragma unroll
+  for (int o = 1; o < kGL; o <<= 1) rank += __shfl_xor_sync(kFullMask, rank, o);
+  return rank;
+}
+// job-level outputs of a placed job; `label` as later_label2 built it (starts after now only)
+__device__ __forceinline__ void write_job2(const JobQ& jq, int64_t start, uint32_t label) {
+  s2_cx.out.start_time[jq.job] = start;
+  s2_cx.out.end_time[jq.job] = start + jq.time_limit;
+  s2_cx.out.n_alloc[jq.job] = jq.node_num;
+  s2_cx.out.reason[jq.job] = start == s2_cx.now ? CRANE_REASON_NONE : later_reason2(label);
+}
+
+// The exact test of node q for an immediate start of the job, in the current state
+// (JobScheduler.cpp:5285-5334): every segment of [now, now + time_limit) holds the
+// request (exclusive: res_total), res_avail itself holds it (:5310) and
+// GetFeasibleResourceInNode passes on res_avail Ckmin'ed with the window. kAlloc:
+// *alloc receives the allocation (exclusive: res_total) of a passing node. By one
+// group; every lane of the warp calls it, a group without work with act = false.
+template <bool kAlloc>
+__device__ __forceinline__ bool g_exact(const JobQ& jq, uint32_t q, bool act, Row* alloc = nullptr) {
+  const TimelineDev& tl = s2_cx.tl;
+  const bool exclusive = jq_exclusive(jq);
+  const uint32_t g = s2_cx.base + (act ? q : 0u);
+  const uint32_t ns = act ? SM2S().nseg[q] : 0u;
+  Row tot, a0;
+  row_zero(tot);
+  row_zero(a0);
+  if (act) {
+    if (exclusive) tot = node_total2(q);
+    else a0 = tl.avail0[g];
+  }
+  Win2 w;
+  g_window(tl.ent + (size_t)g * tl.cap, ns, s2_cx.now + jq.time_limit, jq.req.cpu_raw, jq.req.mem, exclusive, jq_has_gres(jq), tot,
+           act, w);
+  bool ok = act && w.ok;
+  if (exclusive) {
+    if (kAlloc && act) *alloc = tot;
+  } else if (ok) {
+    ok = a0.cpu_raw >= jq.req.cpu_raw && a0.mem >= jq.req.mem;  // res_avail itself (JobScheduler.cpp:5310)
+    if (ok) {
+      Row wr;
+      win_row(w, a0, jq.req, wr);
+      ok = feasible<kAlloc>(jq.req, wr, C_DICT2, alloc);
+    }
+  }
+  return ok;
+}
 
 // Scheduler of several overlapping partitions: membership bytes, one cost array and
 // one order per partition over the shared node states; every NodeSelector starts from
@@ -860,267 +942,15 @@ __device__ __noinline__ void init_orders2(const uint8_t* slot_memb) {
   }
 }
 
-// ---- one job, start to finish (any node_num): JobScheduler.cpp:5224-5404 ----------
-// The walk over the order in windows of 256 positions; every pre-filter
-// candidate is tested exactly (one group each, 32 per round), the first K
-// passing ones are the pick. Fewer than K: backfill on the first K capable nodes.
 // Scheduler with several (overlapping) partitions: the job in hand decides whose order is walked
 __device__ __forceinline__ void enter_partition2(const JobQ& jq) {
   if (s2_cx.ncp > 1) {
     __syncthreads();
     if (threadIdx.x == 0) {
-      s2_curp = (jq.flags >> 16) & 7u;
+      s2_curp = jq_part(jq);
       s2_cx.npos = s2_mcount[s2_curp];
     }
     __syncthreads();
-  }
-}
-
-__device__ __noinline__ void single2(uint32_t ji) {
-  enter_partition2(s2_jobs[ji % s2_cx.ring]);
-  const Smem2 sm = SM2();
-  const uint32_t tid = threadIdx.x, lane = lane_id(), wid = warp_id(), gl = g_lane(), gi = g_index();
-  const uint32_t mp = s2_cx.npos, base = s2_cx.base, ring = s2_cx.ring;
-  const int64_t now = s2_cx.now;
-  const TimelineDev& tl = s2_cx.tl;
-  uint16_t* const list2 = reinterpret_cast<uint16_t*>(sm.scratch);  // first capable nodes
-  const uint32_t slot = ji % ring;
-  mbar_wait(&s2_bar[slot], (ji / ring) & 1u);
-  const JobQ& jq = s2_jobs[slot];
-  JSel2 js;
-  jsel_load(jq, sm.bits_ring + (size_t)slot * s2_cx.words, js);
-  const uint32_t K = jq.node_num;
-  const bool exclusive = js.exclusive;
-  const int64_t limit = jq.time_limit;
-  const View req = jq.req;
-  const int64_t w_end = now + limit;
-  if (K > mp || K == 0) {
-    if (tid == 0) s2_cx.out.reason[jq.job] = CRANE_REASON_RESOURCE;
-    return;
-  }
-  uint32_t nsel = 0, ntot = 0, pos = 0;
-  if (tid == 0) s2_label = 0;
-#ifdef CRANE_PROFILE
-  if (tid == 0) s2_prof_singles += 1;
-#endif
-  while (pos < mp && nsel < K) {
-    // skip a window none of whose blocks can hold a candidate (once the first K
-    // capable nodes are known)
-    if (ntot >= K) {
-      bool any = false;
-      for (uint32_t b = pos / kBlk; b < sm.nblk && b < (pos + kT2) / kBlk; ++b) any = any || block_promising2(sm, js, b);
-      if (!any) { pos += kT2; continue; }
-    }
-    const uint32_t p = pos + tid;
-    uint32_t q = 0;
-    bool cap = false, cand = false;
-    if (p < mp) {
-      q = sm.ord[p];
-      cap = capable2(sm, js, q);
-      cand = cap && prefilter2(sm, js, q);
-    }
-    if (tid == 0) s2_cutpos = pos + kT2;
-    uint32_t totc;
-    const uint32_t rank_c = block_excl_scan(cand ? 1u : 0u, totc);
-    const uint32_t ncand = totc < (uint32_t)kNG ? totc : (uint32_t)kNG;
-#ifdef CRANE_PROFILE
-    if (tid == 0) { s2_prof_windows += 1; s2_prof_tests += ncand; }
-#endif
-    if (cand && rank_c < (uint32_t)kNG) s2_chunk[rank_c] = (uint16_t)q;
-    if (cand && rank_c == (uint32_t)kNG - 1u && totc > (uint32_t)kNG) s2_cutpos = p + 1;  // the rest of the window comes back
-    __syncthreads();
-    const uint32_t cutpos = s2_cutpos;
-    // the first K capable nodes in order: where a backfill goes (JobScheduler.cpp:5269-5278)
-    const bool capc = cap && p < cutpos && ntot < K;
-    uint32_t tott;
-    const uint32_t rank_t = block_excl_scan(capc ? 1u : 0u, tott);
-    if (capc && ntot + rank_t < K) list2[ntot + rank_t] = (uint16_t)q;
-    ntot = ntot + tott < K ? ntot + tott : K;
-    // exact test of the chunk's candidates, one group each
-    {
-      const bool act = gi < ncand;
-      uint32_t qg = 0, g = 0, ns = 0;
-      Row tot, a0;
-      row_zero(tot);
-      row_zero(a0);
-      if (act) {
-        qg = s2_chunk[gi];
-        g = base + qg;
-        ns = sm.nseg[qg];
-        if (exclusive) tot = node_total2(qg);
-        else a0 = tl.avail0[g];
-      }
-      Win2 w;
-      g_window(tl.ent + (size_t)g * tl.cap, ns, w_end, req.cpu_raw, req.mem, exclusive, js.has_gres, tot, act, w);
-      bool ok = act && w.ok;
-      if (ok && !exclusive) {
-        ok = a0.cpu_raw >= req.cpu_raw && a0.mem >= req.mem;  // res_avail itself (JobScheduler.cpp:5310)
-        if (ok) {
-          Row wr;
-          win_row(w, a0, req, wr);
-          ok = feasible<false>(req, wr, C_DICT2, nullptr);
-        }
-      }
-      if (gl == 0) s2_ok[gi] = ok ? 1u : 0u;
-    }
-    __syncthreads();
-    if (wid == 0) {  // the passing ones, in order
-      const bool okl = lane < ncand && s2_ok[lane];
-      const unsigned m = __ballot_sync(kFullMask, okl);
-      const uint32_t r = nsel + (uint32_t)__popc(m & ((1u << lane) - 1u));
-      if (okl && r < K) sm.list[r] = s2_chunk[lane];
-      if (lane == 0) s2_nsel = nsel + (uint32_t)__popc(m) < K ? nsel + (uint32_t)__popc(m) : K;
-    }
-    __syncthreads();
-    nsel = s2_nsel;
-    pos = cutpos;
-  }
-
-  bool placed = false, full_rekey = false;
-  int64_t start_time = now;
-  const uint16_t* nodes = sm.list;
-  if (nsel == K) {
-    // ---- immediate start on list[0..K) (JobScheduler.cpp:5338-5368) ---------
-    placed = true;
-    for (uint32_t k0 = 0; k0 < K; k0 += kNG) {
-      const uint32_t k = k0 + gi;
-      const bool act = k < K;
-      uint32_t q = 0, g = 0, ns = 0;
-      Row tot, a0;
-      row_zero(tot);
-      row_zero(a0);
-      if (act) {
-        q = sm.list[k];
-        g = base + q;
-        ns = sm.nseg[q];
-        if (exclusive) tot = node_total2(q);
-        else a0 = tl.avail0[g];
-      }
-      TlEntry* E = tl.ent + (size_t)g * tl.cap;
-      Win2 w;
-      g_window(E, ns, w_end, req.cpu_raw, req.mem, exclusive, js.has_gres, tot, act, w);
-      Row alloc;
-      row_zero(alloc);
-      if (act) {
-        if (exclusive) alloc = tot;
-        else {
-          Row wr;
-          win_row(w, a0, req, wr);
-          feasible_alloc(req, wr, alloc, s2_cx.dslot);
-        }
-      }
-      Row seg0;
-      row_zero(seg0);
-      const uint32_t nn = g_update(E, ns, now, w_end, alloc, act, seg0);
-      uint32_t rank = 0;  // node-index ascending output slot (deviation D3)
-      if (act && K > 1)
-        for (uint32_t m = gl; m < K; m += kGL) rank += sm.list[m] < q ? 1u : 0u;
-#pragma unroll
-      for (int o = 1; o < kGL; o <<= 1) rank += __shfl_xor_sync(kFullMask, rank, o);
-      if (act && gl == 0) write_node2(jq, q, rank, alloc, nn, seg0);
-    }
-  } else if (ntot >= K) {
-    // ---- backfill on the first K capable nodes: allocation against res_total,
-    // earliest common start (JobScheduler.cpp:5371-5404, JobScheduler.h:806-849)
-    nodes = list2;
-    int64_t T0 = now;
-    bool found = false, failed = false;
-    for (uint32_t it = 0; !found && !failed; ++it) {
-      long long emax = INT64_MIN, emin = kInf;
-      for (uint32_t k0 = 0; k0 < K; k0 += kNG) {
-        const uint32_t k = k0 + gi;
-        const bool act = k < K;
-        uint32_t q = 0, g = 0, ns = 0;
-        Row alloc;
-        row_zero(alloc);
-        if (act) {
-          q = list2[k];
-          g = base + q;
-          ns = sm.nseg[q];
-          const Row tot = node_total2(q);
-          if (exclusive) alloc = tot; else feasible_alloc(req, tot, alloc, s2_cx.dslot);
-        }
-        const int64_t e = g_earliest(tl.ent + (size_t)g * tl.cap, ns, alloc, T0, limit, act);
-        if (act) { emax = e > emax ? e : emax; emin = e < emin ? e : emin; }
-      }
-      if (gl == 0) { s2_e[it & 1u][gi] = emax; s2_e2[it & 1u][gi] = emin; }
-      __syncthreads();
-      long long tmax = INT64_MIN, tmin = kInf;
-      const uint32_t ng = K < (uint32_t)kNG ? K : (uint32_t)kNG;
-      for (uint32_t i = 0; i < ng; ++i) {
-        const long long x = s2_e[it & 1u][i], y = s2_e2[it & 1u][i];
-        tmax = x > tmax ? x : tmax;
-        tmin = y < tmin ? y : tmin;
-      }
-      if (tmax == kInf) failed = true;
-      else if (tmin == tmax) { found = true; T0 = tmax; }  // every node fits from exactly this time on
-      else T0 = tmax;
-    }
-    if (found && T0 - now <= s2_cx.max_window) {  // JobScheduler.h:809
-      placed = true;
-      start_time = T0;
-      for (uint32_t k0 = 0; k0 < K; k0 += kNG) {
-        const uint32_t k = k0 + gi;
-        const bool act = k < K;
-        uint32_t q = 0, g = 0, ns = 0;
-        Row alloc, a0;
-        row_zero(alloc);
-        row_zero(a0);
-        if (act) {
-          q = list2[k];
-          g = base + q;
-          ns = sm.nseg[q];
-          a0 = tl.avail0[g];
-          const Row tot = node_total2(q);
-          if (exclusive) alloc = tot; else feasible_alloc(req, tot, alloc, s2_cx.dslot);
-        }
-        Row seg0;
-        row_zero(seg0);
-        const uint32_t nn = g_update(tl.ent + (size_t)g * tl.cap, ns, T0, T0 + limit, alloc, act, seg0);
-        uint32_t rank = 0;
-        if (act && K > 1)
-          for (uint32_t m = gl; m < K; m += kGL) rank += list2[m] < q ? 1u : 0u;
-#pragma unroll
-        for (int o = 1; o < kGL; o <<= 1) rank += __shfl_xor_sync(kFullMask, rank, o);
-        if (act && gl == 0) {
-          write_node2(jq, q, rank, alloc, nn, seg0);
-          // pending-reason label for future starts (JobScheduler.cpp:5842-5848)
-          if (T0 != now) atomicOr(&s2_label, later_label2(q, !row_le(alloc, a0), limit));
-        }
-      }
-    }
-  }
-  __syncthreads();
-  if (placed) {
-    if (tid == 0) {
-      s2_cx.out.start_time[jq.job] = start_time;
-      s2_cx.out.end_time[jq.job] = start_time + limit;
-      s2_cx.out.n_alloc[jq.job] = K;
-      uint8_t reason = CRANE_REASON_NONE;
-      if (start_time != now) reason = later_reason2(s2_label);
-      s2_cx.out.reason[jq.job] = reason;
-    }
-    // cost += (end-start) * cpu ratio (JobScheduler.h:46-52)
-    full_rekey = K > (uint32_t)kRK;
-    for (uint32_t k = tid; k < K; k += kT2) {
-      const uint32_t q = nodes[k];
-      const double nc = new_cost2(jq, q, sm.cost);
-      if (full_rekey) sm.cost[q] = nc; else { s2_rk_node[k] = q; s2_rk_nc[k] = nc; }
-    }
-  } else if (tid == 0) {
-    s2_cx.out.reason[jq.job] = CRANE_REASON_RESOURCE;  // JobScheduler.cpp:5802
-  }
-  __syncthreads();
-  // list2 lives in the scratch words: back to zero
-  for (uint32_t i = tid; i < (K + 1) / 2 + 1 && i < s2_cx.mp + 4; i += kT2) sm.scratch[i] = 0;
-  __syncthreads();
-  if (placed) {
-    if (full_rekey) order_sort2();
-    else {
-      order_rekey2(K, kT2);
-      __syncthreads();
-      rekey_bounds2(K);
-    }
   }
 }
 
@@ -1139,10 +969,7 @@ __device__ __noinline__ void single2(uint32_t ji) {
 // everything in front of a pick is either listed (tested) or fails the pre-filter.
 __shared__ uint32_t s2_vok[kMaxJ], s2_voff[kMaxJ + 1];
 __device__ __noinline__ void validate2(uint32_t nj) {
-  const Smem2 sm = SM2S();
   const uint32_t tid = threadIdx.x, lane = lane_id(), gl = g_lane(), gi = g_index();
-  const TimelineDev& tl = s2_cx.tl;
-  const int64_t now = s2_cx.now;
   if (tid < 32) {  // pairs per job, exclusive prefix
     uint32_t c = 0;
     if (lane < nj) {
@@ -1179,31 +1006,7 @@ __device__ __noinline__ void validate2(uint32_t nj) {
       t = best ? best - 1u : 0u;
     }
     const uint32_t e = act ? x - s2_voff[t] : 0u;
-    const JobQ& jq = s2_jobs[s2_bj[t].slot];
-    const bool exclusive = jq.flags & 1u;
-    const View req = jq.req;
-    uint32_t q = 0, g = s2_cx.base, ns = 0;
-    Row tot, a0;
-    row_zero(tot);
-    row_zero(a0);
-    if (act) {
-      q = s2_cl[0][t][e];
-      g = s2_cx.base + q;
-      ns = sm.nseg[q];
-      if (exclusive) tot = node_total2(q);
-      else a0 = tl.avail0[g];
-    }
-    Win2 w;
-    g_window(tl.ent + (size_t)g * tl.cap, ns, now + jq.time_limit, req.cpu_raw, req.mem, exclusive, (jq.flags & 2u) != 0, tot, act, w);
-    bool ok = act && w.ok;
-    if (ok && !exclusive) {
-      ok = a0.cpu_raw >= req.cpu_raw && a0.mem >= req.mem;  // res_avail itself (JobScheduler.cpp:5310)
-      if (ok) {
-        Row wr;
-        win_row(w, a0, req, wr);
-        ok = feasible<false>(req, wr, C_DICT2, nullptr);
-      }
-    }
+    const bool ok = g_exact<false>(s2_jobs[s2_bj[t].slot], act ? s2_cl[0][t][e] : 0u, act);
     if (ok && gl == 0) atomicOr(&s2_vok[t], 1u << e);
   }
   __syncthreads();
@@ -1255,7 +1058,7 @@ struct Heap2 {
   uint32_t size, sum;
 };
 __shared__ Heap2 s2_heap[2];                 // [0] by res_total (backfill), [1] by the window minimum (immediate start)
-__shared__ uint16_t s2_g_nt[2][kNG];         // per chunk candidate: tasks by res_total / by the window minimum
+__shared__ uint16_t s2_g_nt[2][kNG];         // per window candidate: tasks by res_total / by the window minimum
 __shared__ uint16_t s2_g_node[kHeapMax], s2_g_n[kHeapMax];  // hand-out: node, tasks, in pop order
 __shared__ uint32_t s2_g_done;
 
@@ -1311,10 +1114,19 @@ __device__ __noinline__ uint32_t max_tasks2(const View& min_view, const View& re
   return n;
 }
 
-__device__ __noinline__ void single2_general(uint32_t ji) {
+// ---- the one-job path: one job, start to finish (any node_num), JobScheduler.cpp:5224-5404 ----
+// The walk over the order in windows of 256 positions; up to 32 candidates of a
+// window are tested at once, one group each. Uniform tasks (kGeneral = false): the
+// candidates are the pre-filter ones, each gets the exact test, the first K passing
+// ones are the pick and with fewer than K the job backfills on the first K capable
+// nodes. General task distribution: every capable node counts the tasks it can take
+// by res_total and by the window minimum into the two heaps above, which decide.
+// Both then share the earliest common start, the placement and the job tail.
+template <bool kGeneral>
+__device__ __noinline__ void single2(uint32_t ji) {
   enter_partition2(s2_jobs[ji % s2_cx.ring]);
   const Smem2 sm = SM2();
-  const uint32_t tid = threadIdx.x, lane = lane_id(), wid = warp_id(), gl = g_lane(), gi = g_index();
+  const uint32_t tid = threadIdx.x, gl = g_lane(), gi = g_index();
   const uint32_t mp = s2_cx.npos, base = s2_cx.base, ring = s2_cx.ring;
   const int64_t now = s2_cx.now;
   const TimelineDev& tl = s2_cx.tl;
@@ -1323,299 +1135,275 @@ __device__ __noinline__ void single2_general(uint32_t ji) {
   const JobQ& jq = s2_jobs[slot];
   JSel2 js;
   jsel_load(jq, sm.bits_ring + (size_t)slot * s2_cx.words, js);
-  const uint32_t K = jq.node_num, tmin = jq.ntasks_per_node, tmax = jq.ntpn_max, ntasks = jq.ntasks;
+  const uint32_t K = jq.node_num;
   const bool exclusive = js.exclusive;
   const int64_t limit = jq.time_limit;
-  const View min_view = jq.req;
-  const View req_node = s2_cx.req_node[jq.job], req_task = s2_cx.req_task[jq.job];
+  const View req = jq.req;  // general task distribution: what a node needs at least (min_res_view)
   const int64_t w_end = now + limit;
-  if (K > mp || K == 0 || K >= (uint32_t)kHeapMax) {
+  // general task distribution: a node with n tasks needs req_node + n * req_task
+  const View req_node = kGeneral ? s2_cx.req_node[jq.job] : req, req_task = kGeneral ? s2_cx.req_task[jq.job] : req;
+  const uint32_t tmin = jq.ntasks_per_node, tmax = jq.ntpn_max, ntasks = jq.ntasks;
+  if (K > mp || K == 0 || (kGeneral && K >= (uint32_t)kHeapMax)) {
     if (tid == 0) s2_cx.out.reason[jq.job] = CRANE_REASON_RESOURCE;
     return;
   }
-  if (tid == 0) { s2_heap[0].size = 0; s2_heap[0].sum = 0; s2_heap[1].size = 0; s2_heap[1].sum = 0; s2_g_done = 0; s2_label = 0; }
-  __syncthreads();
-  // ---- the walk: capable nodes in order, 32 per round --------------------------------
-  uint32_t pos = 0;
-  while (pos < mp && !s2_g_done) {
+  uint16_t* const list2 = reinterpret_cast<uint16_t*>(sm.scratch);  // uniform tasks: the first K capable nodes
+  uint32_t nsel = 0, ntot = 0, pos = 0;
+  if (tid == 0) {
+    s2_label = 0;
+    if (kGeneral) { s2_heap[0].size = 0; s2_heap[0].sum = 0; s2_heap[1].size = 0; s2_heap[1].sum = 0; s2_g_done = 0; }
+  }
+  if (kGeneral) __syncthreads();
+#ifdef CRANE_PROFILE
+  if (!kGeneral && tid == 0) s2_prof_singles += 1;
+#endif
+  while (pos < mp && (kGeneral ? !s2_g_done : nsel < K)) {
+    // skip a window none of whose blocks can hold a candidate (once the first K
+    // capable nodes are known)
+    if (!kGeneral && ntot >= K) {
+      bool any = false;
+      for (uint32_t b = pos / kBlk; b < sm.nblk && b < (pos + kT2) / kBlk; ++b) any = any || block_promising2(sm, js, b);
+      if (!any) { pos += kT2; continue; }
+    }
     const uint32_t p = pos + tid;
     uint32_t q = 0;
-    bool cap = false;
+    bool cap = false, cand = false;
     if (p < mp) {
       q = sm.ord[p];
       cap = capable2(sm, js, q);
+      cand = cap && (kGeneral || prefilter2(sm, js, q));
     }
     if (tid == 0) s2_cutpos = pos + kT2;
     uint32_t totc;
-    const uint32_t rank_c = block_excl_scan(cap ? 1u : 0u, totc);
+    const uint32_t rank_c = block_excl_scan(cand ? 1u : 0u, totc);
     const uint32_t ncand = totc < (uint32_t)kNG ? totc : (uint32_t)kNG;
-    if (cap && rank_c < (uint32_t)kNG) s2_chunk[rank_c] = (uint16_t)q;
-    if (cap && rank_c == (uint32_t)kNG - 1u && totc > (uint32_t)kNG) s2_cutpos = p + 1;
+#ifdef CRANE_PROFILE
+    if (!kGeneral && tid == 0) { s2_prof_windows += 1; s2_prof_tests += ncand; }
+#endif
+    if (cand && rank_c < (uint32_t)kNG) s2_chunk[rank_c] = (uint16_t)q;
+    if (cand && rank_c == (uint32_t)kNG - 1u && totc > (uint32_t)kNG) s2_cutpos = p + 1;  // the rest of the window comes back
     __syncthreads();
     const uint32_t cutpos = s2_cutpos;
-    {
+    if constexpr (kGeneral) {
+      // tasks every candidate can take by res_total and by the window minimum
+      // (JobScheduler.cpp:5258-5334), one group each
       const bool act = gi < ncand;
       uint32_t qg = 0, g = 0, ns = 0;
       Row tot, a0;
       row_zero(tot);
       row_zero(a0);
+      bool fits = false;  // res_avail holds the minimum (JobScheduler.cpp:5310)
       if (act) {
         qg = s2_chunk[gi];
         g = base + qg;
         ns = sm.nseg[qg];
         tot = node_total2(qg);
         a0 = tl.avail0[g];
+        fits = !exclusive && feasible<false>(req, a0, C_DICT2, nullptr);
       }
       Win2 w;
-      g_window(tl.ent + (size_t)g * tl.cap, ns, w_end, min_view.cpu_raw, min_view.mem, true, false, tot, act && exclusive, w);
+      g_window<true>(tl.ent + (size_t)g * tl.cap, ns, w_end, req.cpu_raw, req.mem, exclusive, true, tot, act && (exclusive || fits), w);
       if (act && gl == 0) {
-        const uint32_t n_total = max_tasks2(min_view, req_task, tmin, tmax, tot);  // > 0: the node is capable
+        const uint32_t n_total = max_tasks2(req, req_task, tmin, tmax, tot);  // > 0: the node is capable
+        uint32_t n_avail = 0;
+        if (exclusive) {
+          n_avail = w.ok ? n_total : 0u;  // JobScheduler.cpp:5285-5307
+        } else if (fits) {
+          Row wr;
+          win_row_min(w, a0, req, wr);
+          n_avail = max_tasks2(req, req_task, tmin, tmax, wr);
+        }
         s2_g_nt[0][gi] = (uint16_t)n_total;
-        if (exclusive) s2_g_nt[1][gi] = w.ok ? (uint16_t)n_total : (uint16_t)0;  // JobScheduler.cpp:5285-5307
-        else s2_g_nt[1][gi] = feasible<false>(min_view, a0, C_DICT2, nullptr) ? (uint16_t)0xffffu : (uint16_t)0;  // :5310; 0xffff = to be counted below
+        s2_g_nt[1][gi] = (uint16_t)n_avail;
       }
-    }
-    __syncthreads();
-    // the window minimum row itself (cpu, mem minima too) for the candidates that need it
-    {
-      const bool act = gi < ncand && s2_g_nt[1][gi] == 0xffffu;
-      uint32_t qg = 0, g = 0, ns = 0;
-      if (act) { qg = s2_chunk[gi]; g = base + qg; ns = sm.nseg[qg]; }
-      const TlEntry* E = tl.ent + (size_t)g * tl.cap;
-      long long mcpu = INT64_MAX;
-      unsigned long long mmem = ~0ull, msw = ~0ull;
-      bool more = act;
-      for (uint32_t b0 = 0; __any_sync(kFullMask, more); b0 += kGL) {
-        const uint32_t i = b0 + gl;
-        bool inw = false;
-        if (more && i < ns) {
-          const TlEntry e = E[i];
-          inw = e.t < w_end;
-          if (inw) {
-            mcpu = e.seg.cpu_raw < mcpu ? e.seg.cpu_raw : mcpu;
-            mmem = e.seg.mem < mmem ? e.seg.mem : mmem;
-            msw = e.seg.mem_sw < msw ? e.seg.mem_sw : msw;
+      __syncthreads();
+      // heaps, in node order (one thread: the reference's loop body, JobScheduler.cpp:5269-5334)
+      if (tid == 0) {
+        Heap2& ht = s2_heap[0];
+        Heap2& ha = s2_heap[1];
+        for (uint32_t c = 0; c < ncand; ++c) {
+          const uint32_t n_total = s2_g_nt[0][c], n_avail = s2_g_nt[1][c], qn = s2_chunk[c];
+          if (n_total == 0) continue;
+          if (ht.size < K || ht.sum < ntasks) {
+            ht.sum += n_total;
+            heap_push2(ht, n_total, qn);
+            if (ht.size > K) { ht.sum -= ht.nt[0]; heap_pop2(ht); }
+          }
+          if (n_avail) {
+            ha.sum += n_avail;
+            heap_push2(ha, n_avail, qn);
+            if (ha.size > K) { ha.sum -= ha.nt[0]; heap_pop2(ha); }
+            if (ha.size == K && ha.sum >= ntasks) { s2_g_done = 1; break; }
           }
         }
-        if (g_ballot(inw) != (1u << kGL) - 1u) more = false;
       }
-#pragma unroll
-      for (int o = 1; o < kGL; o <<= 1) {
-        const long long oc = __shfl_xor_sync(kFullMask, mcpu, o);
-        const unsigned long long om = __shfl_xor_sync(kFullMask, mmem, o), os = __shfl_xor_sync(kFullMask, msw, o);
-        mcpu = oc < mcpu ? oc : mcpu;
-        mmem = om < mmem ? om : mmem;
-        msw = os < msw ? os : msw;
+      __syncthreads();
+    } else {
+      // the first K capable nodes in order: where a backfill goes (JobScheduler.cpp:5269-5278)
+      const bool capc = cap && p < cutpos && ntot < K;
+      uint32_t tott;
+      const uint32_t rank_t = block_excl_scan(capc ? 1u : 0u, tott);
+      if (capc && ntot + rank_t < K) list2[ntot + rank_t] = (uint16_t)q;
+      ntot = ntot + tott < K ? ntot + tott : K;
+      // the exact test of the window's candidates, one group each
+      const bool act = gi < ncand;
+      const bool ok = g_exact<false>(jq, act ? s2_chunk[gi] : 0u, act);
+      if (gl == 0) s2_ok[gi] = ok ? 1u : 0u;
+      __syncthreads();
+      if (warp_id() == 0) {  // the passing ones, in order
+        const uint32_t lane = lane_id();
+        const bool okl = lane < ncand && s2_ok[lane];
+        const unsigned m = __ballot_sync(kFullMask, okl);
+        const uint32_t r = nsel + (uint32_t)__popc(m & ((1u << lane) - 1u));
+        if (okl && r < K) sm.list[r] = s2_chunk[lane];
+        if (lane == 0) s2_nsel = nsel + (uint32_t)__popc(m) < K ? nsel + (uint32_t)__popc(m) : K;
       }
-      Win2 w;
-      Row tot;
-      row_zero(tot);
-      g_window(E, ns, w_end, min_view.cpu_raw, min_view.mem, false, true, tot, act, w);
-      if (act && gl == 0) {
-        const Row a0 = tl.avail0[g];
-        Row wr;
-        win_row(w, a0, min_view, wr);
-        wr.cpu_raw = a0.cpu_raw < mcpu ? a0.cpu_raw : mcpu;  // res_avail Ckmin'ed with every segment of the window
-        wr.mem = a0.mem < mmem ? a0.mem : mmem;
-        wr.mem_sw = a0.mem_sw < msw ? a0.mem_sw : msw;
-        s2_g_nt[1][gi] = (uint16_t)max_tasks2(min_view, req_task, tmin, tmax, wr);
-      }
+      __syncthreads();
+      nsel = s2_nsel;
     }
-    __syncthreads();
-    // heaps, in node order (one thread: the reference's loop body, JobScheduler.cpp:5269-5334)
-    if (tid == 0) {
-      Heap2& ht = s2_heap[0];
-      Heap2& ha = s2_heap[1];
-      for (uint32_t c = 0; c < ncand; ++c) {
-        const uint32_t n_total = s2_g_nt[0][c], n_avail = s2_g_nt[1][c], qn = s2_chunk[c];
-        if (n_total == 0) continue;
-        if (ht.size < K || ht.sum < ntasks) {
-          ht.sum += n_total;
-          heap_push2(ht, n_total, qn);
-          if (ht.size > K) { ht.sum -= ht.nt[0]; heap_pop2(ht); }
-        }
-        if (n_avail) {
-          ha.sum += n_avail;
-          heap_push2(ha, n_avail, qn);
-          if (ha.size > K) { ha.sum -= ha.nt[0]; heap_pop2(ha); }
-          if (ha.size == K && ha.sum >= ntasks) { s2_g_done = 1; break; }
-        }
-      }
-    }
-    __syncthreads();
     pos = cutpos;
   }
-  // ---- decision and hand-out (JobScheduler.cpp:5338-5404) ---------------------------------
-  const bool start_now = s2_heap[1].size == K && s2_heap[1].sum >= ntasks;
-  const bool can_bf = s2_heap[0].size == K && s2_heap[0].sum >= ntasks;
-  __syncthreads();
-  if (tid == 0 && (start_now || can_bf)) {
-    Heap2& h = s2_heap[start_now ? 1 : 0];
-    int32_t rest = (int32_t)ntasks - (int32_t)K;
-    uint32_t k = 0;
-    while (h.size) {
-      const int32_t cap_n = (int32_t)h.nt[0] - 1;
-      const int32_t n = (rest < cap_n ? rest : cap_n) + 1;
-      s2_g_node[k] = h.q[0];
-      s2_g_n[k] = (uint16_t)n;
-      rest -= n - 1;
-      ++k;
-      heap_pop2(h);
-    }
-  }
-  __syncthreads();
-  bool placed = false;
-  int64_t start_time = now;
-  if (start_now || can_bf) {
-    int64_t T0 = now;
-    bool ok = true;
-    if (!start_now) {
-      // earliest common start of the K nodes (JobScheduler.h:806-849), allocation against res_total
-      bool found = false, failed = false;
-      for (uint32_t it = 0; !found && !failed; ++it) {
-        long long emax = INT64_MIN, emin = kInf;
-        for (uint32_t k0 = 0; k0 < K; k0 += kNG) {
-          const uint32_t k = k0 + gi;
-          const bool act = k < K;
-          uint32_t q = 0, g = 0, ns = 0;
-          Row alloc;
-          row_zero(alloc);
-          if (act) {
-            q = s2_g_node[k];
-            g = base + q;
-            ns = sm.nseg[q];
-            const Row tot = node_total2(q);
-            if (exclusive) alloc = tot;
-            else { View full; view_node_plus_tasks(full, req_node, req_task, s2_g_n[k]); feasible_alloc(full, tot, alloc, s2_cx.dslot); }
-          }
-          const int64_t e = g_earliest(tl.ent + (size_t)g * tl.cap, ns, alloc, T0, limit, act);
-          if (act) { emax = e > emax ? e : emax; emin = e < emin ? e : emin; }
-        }
-        if (gl == 0) { s2_e[it & 1u][gi] = emax; s2_e2[it & 1u][gi] = emin; }
-        __syncthreads();
-        long long tmx = INT64_MIN, tmn = kInf;
-        const uint32_t ng = K < (uint32_t)kNG ? K : (uint32_t)kNG;
-        for (uint32_t i = 0; i < ng; ++i) {
-          const long long x = s2_e[it & 1u][i], y = s2_e2[it & 1u][i];
-          tmx = x > tmx ? x : tmx;
-          tmn = y < tmn ? y : tmn;
-        }
-        if (tmx == kInf) failed = true;
-        else if (tmn == tmx) { found = true; T0 = tmx; }
-        else T0 = tmx;
+
+  // ---- the decision (JobScheduler.cpp:5338-5404): start now on `nodes`, or backfill on them
+  bool start_now, can_bf;
+  const uint16_t* nodes;
+  if constexpr (kGeneral) {
+    start_now = s2_heap[1].size == K && s2_heap[1].sum >= ntasks;
+    can_bf = s2_heap[0].size == K && s2_heap[0].sum >= ntasks;
+    __syncthreads();
+    if (tid == 0 && (start_now || can_bf)) {  // hand-out: tasks in pop order
+      Heap2& h = s2_heap[start_now ? 1 : 0];
+      int32_t rest = (int32_t)ntasks - (int32_t)K;
+      uint32_t k = 0;
+      while (h.size) {
+        const int32_t cap_n = (int32_t)h.nt[0] - 1;
+        const int32_t n = (rest < cap_n ? rest : cap_n) + 1;
+        s2_g_node[k] = h.q[0];
+        s2_g_n[k] = (uint16_t)n;
+        rest -= n - 1;
+        ++k;
+        heap_pop2(h);
       }
-      ok = found && T0 - now <= s2_cx.max_window;
     }
-    if (ok) {
-      placed = true;
-      start_time = T0;
+    __syncthreads();
+    nodes = s2_g_node;
+  } else {
+    start_now = nsel == K;
+    can_bf = ntot >= K;
+    nodes = start_now ? sm.list : list2;
+  }
+  // the allocation of node k out of `src`
+  auto alloc_from = [&](uint32_t k, const Row& src, Row& alloc) {
+    if constexpr (kGeneral) {
+      View full;
+      view_node_plus_tasks(full, req_node, req_task, s2_g_n[k]);
+      feasible_alloc(full, src, alloc, s2_cx.dslot);
+    } else {
+      feasible_alloc(req, src, alloc, s2_cx.dslot);
+    }
+  };
+  int64_t T0 = now;
+  bool placed = start_now;
+  if (!start_now && can_bf) {
+    // earliest common start of the K nodes, allocation against res_total (JobScheduler.cpp:5371-5404,
+    // JobScheduler.h:806-849): T <- max over the nodes of their earliest fit >= T, to the fixed point
+    bool found = false, failed = false;
+    for (uint32_t it = 0; !found && !failed; ++it) {
+      long long emax = INT64_MIN, emin = kInf;
       for (uint32_t k0 = 0; k0 < K; k0 += kNG) {
         const uint32_t k = k0 + gi;
         const bool act = k < K;
         uint32_t q = 0, g = 0, ns = 0;
-        Row tot, a0;
-        row_zero(tot);
-        row_zero(a0);
-        if (act) {
-          q = s2_g_node[k];
-          g = base + q;
-          ns = sm.nseg[q];
-          tot = node_total2(q);
-          a0 = tl.avail0[g];
-        }
-        TlEntry* E = tl.ent + (size_t)g * tl.cap;
-        // the window minimum again (immediate start: the allocation comes out of it)
-        long long mcpu = INT64_MAX;
-        unsigned long long mmem = ~0ull, msw = ~0ull;
-        bool more = act && start_now && !exclusive;
-        for (uint32_t b0 = 0; __any_sync(kFullMask, more); b0 += kGL) {
-          const uint32_t i = b0 + gl;
-          bool inw = false;
-          if (more && i < ns) {
-            const TlEntry e = E[i];
-            inw = e.t < w_end;
-            if (inw) {
-              mcpu = e.seg.cpu_raw < mcpu ? e.seg.cpu_raw : mcpu;
-              mmem = e.seg.mem < mmem ? e.seg.mem : mmem;
-              msw = e.seg.mem_sw < msw ? e.seg.mem_sw : msw;
-            }
-          }
-          if (g_ballot(inw) != (1u << kGL) - 1u) more = false;
-        }
-#pragma unroll
-        for (int o = 1; o < kGL; o <<= 1) {
-          const long long oc = __shfl_xor_sync(kFullMask, mcpu, o);
-          const unsigned long long om = __shfl_xor_sync(kFullMask, mmem, o), os = __shfl_xor_sync(kFullMask, msw, o);
-          mcpu = oc < mcpu ? oc : mcpu;
-          mmem = om < mmem ? om : mmem;
-          msw = os < msw ? os : msw;
-        }
-        Win2 w;
-        g_window(E, ns, w_end, min_view.cpu_raw, min_view.mem, false, true, tot, act && start_now && !exclusive, w);
         Row alloc;
         row_zero(alloc);
         if (act) {
-          if (exclusive) alloc = tot;
-          else {
-            View full;
-            view_node_plus_tasks(full, req_node, req_task, s2_g_n[k]);
-            Row src = tot;
-            if (start_now) {
-              win_row(w, a0, min_view, src);
-              src.cpu_raw = a0.cpu_raw < mcpu ? a0.cpu_raw : mcpu;
-              src.mem = a0.mem < mmem ? a0.mem : mmem;
-              src.mem_sw = a0.mem_sw < msw ? a0.mem_sw : msw;
-            }
-            feasible_alloc(full, src, alloc, s2_cx.dslot);
-          }
+          q = nodes[k];
+          g = base + q;
+          ns = sm.nseg[q];
+          const Row tot = node_total2(q);
+          if (exclusive) alloc = tot; else alloc_from(k, tot, alloc);
         }
-        Row seg0;
-        row_zero(seg0);
-        const uint32_t nn = g_update(E, ns, T0, T0 + limit, alloc, act, seg0);
-        uint32_t rank = 0;  // node-index ascending output slot (deviation D3)
-        if (act && K > 1)
-          for (uint32_t m = gl; m < K; m += kGL) rank += s2_g_node[m] < q ? 1u : 0u;
-#pragma unroll
-        for (int o = 1; o < kGL; o <<= 1) rank += __shfl_xor_sync(kFullMask, rank, o);
-        if (act && gl == 0) {
-          write_node2(jq, q, rank, alloc, nn, seg0);
-          s2_cx.out.alloc_ntasks[jq.alloc_off + rank] = s2_g_n[k];
-          if (T0 != now) atomicOr(&s2_label, later_label2(q, !row_le(alloc, a0), limit));
+        const int64_t e = g_earliest(tl.ent + (size_t)g * tl.cap, ns, alloc, T0, limit, act);
+        if (act) { emax = e > emax ? e : emax; emin = e < emin ? e : emin; }
+      }
+      if (gl == 0) { s2_e[it & 1u][gi] = emax; s2_e2[it & 1u][gi] = emin; }
+      __syncthreads();
+      long long hi = INT64_MIN, lo = kInf;
+      const uint32_t ng = K < (uint32_t)kNG ? K : (uint32_t)kNG;
+      for (uint32_t i = 0; i < ng; ++i) {
+        const long long x = s2_e[it & 1u][i], y = s2_e2[it & 1u][i];
+        hi = x > hi ? x : hi;
+        lo = y < lo ? y : lo;
+      }
+      if (hi == kInf) failed = true;
+      else if (lo == hi) { found = true; T0 = hi; }  // every node fits from exactly this time on
+      else T0 = hi;
+    }
+    placed = found && T0 - now <= s2_cx.max_window;  // JobScheduler.h:809
+  }
+  if (placed) {
+    // ---- the K nodes from T0 on: allocation, timeline update, outputs
+    for (uint32_t k0 = 0; k0 < K; k0 += kNG) {
+      const uint32_t k = k0 + gi;
+      const bool act = k < K;
+      const uint32_t q = act ? nodes[k] : 0u, g = base + q, ns = act ? sm.nseg[q] : 0u;
+      TlEntry* E = tl.ent + (size_t)g * tl.cap;
+      Row alloc;
+      row_zero(alloc);
+      if (!kGeneral && start_now) {
+        g_exact<true>(jq, q, act, &alloc);  // out of the window (the node passed this test in the walk)
+      } else {
+        Row tot;
+        row_zero(tot);
+        if (act) tot = node_total2(q);
+        Row src = tot;
+        if (kGeneral && start_now) {  // out of the window minimum
+          Win2 w;
+          g_window<true>(E, ns, w_end, req.cpu_raw, req.mem, false, true, tot, act && !exclusive, w);
+          if (act && !exclusive) win_row_min(w, tl.avail0[g], req, src);
         }
+        if (act) { if (exclusive) alloc = tot; else alloc_from(k, src, alloc); }
+      }
+      Row seg0;
+      row_zero(seg0);
+      const uint32_t nn = g_update(E, ns, T0, T0 + limit, alloc, act, seg0);
+      const uint32_t rank = g_out_rank(K, q, act, [&](uint32_t m) { return (uint32_t)nodes[m]; });
+      if (act && gl == 0) {
+        write_node2(jq, q, rank, alloc, nn, seg0);
+        if (kGeneral) s2_cx.out.alloc_ntasks[jq.alloc_off + rank] = s2_g_n[k];
+        // pending-reason label for future starts (JobScheduler.cpp:5842-5848)
+        if (T0 != now) atomicOr(&s2_label, later_label2(q, !row_le(alloc, tl.avail0[g]), limit));
       }
     }
   }
   __syncthreads();
+  const bool full_rekey = K > (uint32_t)kRK;
   if (placed) {
-    if (tid == 0) {
-      s2_cx.out.start_time[jq.job] = start_time;
-      s2_cx.out.end_time[jq.job] = start_time + limit;
-      s2_cx.out.n_alloc[jq.job] = K;
-      uint8_t reason = CRANE_REASON_NONE;
-      if (start_time != now) reason = later_reason2(s2_label);
-      s2_cx.out.reason[jq.job] = reason;
-    }
-    // the node's cost grows by its own allocation's cpu share (JobScheduler.h:46-52)
-    const bool full_rekey = K > (uint32_t)kRK;
+    if (tid == 0) write_job2(jq, T0, s2_label);
+    // the node's cost grows by its allocation's cpu share (JobScheduler.h:46-52)
     for (uint32_t k = tid; k < K; k += kT2) {
-      const uint32_t q = s2_g_node[k];
+      const uint32_t q = nodes[k];
       const int64_t tot_cpu = node_total_cpu2(q);
-      const int64_t cpu = exclusive ? tot_cpu : req_node.cpu_raw + req_task.cpu_raw * (int64_t)s2_g_n[k];
+      const int64_t cpu = exclusive ? tot_cpu : kGeneral ? req_node.cpu_raw + req_task.cpu_raw * (int64_t)s2_g_n[k] : req.cpu_raw;
       const double nc = __dadd_rn(sm.cost[q], cost_step(s2_cx.cost_policy, limit, cpu, tot_cpu));
       if (full_rekey) sm.cost[q] = nc; else { s2_rk_node[k] = q; s2_rk_nc[k] = nc; }
     }
+  } else if (tid == 0) {
+    s2_cx.out.reason[jq.job] = CRANE_REASON_RESOURCE;  // JobScheduler.cpp:5802
+  }
+  if (!kGeneral) {  // list2 lives in the scratch words: back to zero
     __syncthreads();
+    for (uint32_t i = tid; i < (K + 1) / 2 + 1 && i < s2_cx.mp + 4; i += kT2) sm.scratch[i] = 0;
+  }
+  __syncthreads();
+  if (placed) {
     if (full_rekey) order_sort2();
     else {
       order_rekey2(K, kT2);
       __syncthreads();
       rekey_bounds2(K);
     }
-  } else if (tid == 0) {
-    s2_cx.out.reason[jq.job] = CRANE_REASON_RESOURCE;  // JobScheduler.cpp:5802
   }
-  (void)wid;
-  (void)lane;
 }
 
 __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
@@ -1691,7 +1479,7 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
     if (want_single) {
       if (wid == 0 && lane == 0) mbar_wait(&s2_bar[ji % ring], (ji / ring) & 1u);
       __syncthreads();
-      if (s2_jobs[ji % ring].flags & 4u) single2_general(ji); else single2(ji);
+      if (jq_general(s2_jobs[ji % ring])) single2<true>(ji); else single2<false>(ji);
       PROF(7);
       ++ji;
       want_single = s2_cx.ncp > 1;
@@ -1707,7 +1495,7 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
         myslot = j % ring;
         mbar_wait(&s2_bar[myslot], (j / ring) & 1u);
         myK = s2_jobs[myslot].node_num;
-        okj = myK >= 1 && myK <= mp && myK <= (uint32_t)kMaxT && !(s2_jobs[myslot].flags & 4u);
+        okj = myK >= 1 && myK <= mp && myK <= (uint32_t)kMaxT && !jq_general(s2_jobs[myslot]);
       }
       uint32_t cum = okj ? myK : (uint32_t)kMaxT + 1u;
       for (int o = 1; o < 32; o <<= 1) {
@@ -1799,7 +1587,7 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
       tjq = &s2_jobs[s2_bj[tjob].slot];
       tK = jw & 0xffu; tfirst = (jw >> 8) & 0xffu; tmode = (jw >> 16) & 1u; tstate = (jw >> 17) & 3u;
     }
-    const bool texcl = tjq->flags & 1u;
+    const bool texcl = jq_exclusive(*tjq);
     const int64_t tlimit = tjq->time_limit;
     uint32_t njr = nj, NT = 0;
     bool tact = false;
@@ -1880,7 +1668,7 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
           __syncwarp();
           if (tv != 0xffffu) sm.scratch[tv] = 0;  // the marks go back to zero
           if (lane == 0) { s2_njr = njr_l; s2_cut = NTl; }
-        } else if (CRANE_SPEC_EVAL && myslot < nslots && tstate == 0) {
+        } else if (myslot < nslots && tstate == 0) {
           // first guess of my slot: entry `myslot` of the job's list if the list is
           // long enough for all the jobs before it to be served, else its own i-th entry
           const uint32_t jw = s2_jw[tjob];
@@ -1910,7 +1698,7 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
           if (texcl || tmode) etot = node_total2(q);
         }
         Win2 w;
-        g_window(E, ns, now + tlimit, tjq->req.cpu_raw, tjq->req.mem, texcl, (tjq->flags & 2u) != 0, etot, do_eval && !tmode, w);
+        g_window(E, ns, now + tlimit, tjq->req.cpu_raw, tjq->req.mem, texcl, jq_has_gres(*tjq), etot, do_eval && !tmode, w);
         if (do_eval && !tmode) {
           tok = w.ok;
           if (texcl) talloc = etot;
@@ -2003,11 +1791,7 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
       Row seg0;
       row_zero(seg0);
       const uint32_t nn = g_update(tE, tns, start, start + tlimit, talloc, cact, seg0);
-      uint32_t rank = 0;  // node-index ascending output slot (deviation D3)
-      if (cact && tK > 1)
-        for (uint32_t m = gl; m < tK; m += kGL) rank += s2_task[tfirst + m].q < tq ? 1u : 0u;
-#pragma unroll
-      for (int o = 1; o < kGL; o <<= 1) rank += __shfl_xor_sync(kFullMask, rank, o);
+      const uint32_t rank = g_out_rank(tK, tq, cact, [&](uint32_t m) { return s2_task[tfirst + m].q; });
       if (cact && gl == 0) {
         write_node2(*tjq, tq, rank, talloc, nn, seg0);
         if (start != now) atomicOr(&s2_joblabel[tjob], later_label2(tq, tshort, tlimit));
@@ -2030,15 +1814,8 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
     if (tid < done) {
       const BJob2 b = s2_bj[tid];
       const JobQ& jq = s2_jobs[b.slot];
-      if (b.state == 2u) {
-        a.out.reason[jq.job] = CRANE_REASON_RESOURCE;
-      } else {
-        const int64_t st = b.mode ? (int64_t)s2_T0[tid] : now;
-        a.out.start_time[jq.job] = st;
-        a.out.end_time[jq.job] = st + jq.time_limit;
-        a.out.n_alloc[jq.job] = b.K;
-        a.out.reason[jq.job] = st == now ? CRANE_REASON_NONE : later_reason2(s2_joblabel[tid]);
-      }
+      if (b.state == 2u) a.out.reason[jq.job] = CRANE_REASON_RESOURCE;
+      else write_job2(jq, b.mode ? (int64_t)s2_T0[tid] : now, s2_joblabel[tid]);
     }
     if (fjob != 0xffffffffu) {
       const BJob2 b = s2_bj[fjob];

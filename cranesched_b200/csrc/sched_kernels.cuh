@@ -137,7 +137,7 @@ struct __align__(16) JobQ {
   uint32_t node_num;
   uint32_t alloc_off;
   uint32_t ntasks_per_node;
-  uint32_t flags;      // bit0 exclusive, bit1 has gres request, bit2 general task distribution, bits 8-15 requested gres names
+  uint32_t flags;      // kJq* below
   uint32_t ntpn_max;   // ntasks_per_node_max
   uint64_t spec8;      // per-entry typed counts, one byte each (clamped to 127)
   uint8_t name_need[CRANE_GRES_NAMES];  // per name max(total, sum typed), clamped to 255
@@ -145,6 +145,17 @@ struct __align__(16) JobQ {
   uint32_t vpart;      // scheduler of the job: partition, or n_parts + reservation
 };
 static_assert(sizeof(JobQ) == 112, "JobQ layout");
+// JobQ::flags
+constexpr uint32_t kJqExclusive = 1u << 0;  // exclusive node allocation
+constexpr uint32_t kJqHasGres = 1u << 1;    // the request names gres
+constexpr uint32_t kJqGeneral = 1u << 2;    // general task distribution (a ntasks_per_node range or an uneven ntasks)
+constexpr uint32_t kJqNamesShift = 8;       // bits 8-15: gres names requested (bit per name)
+constexpr uint32_t kJqPartShift = 16;       // bits 16-18: partition inside a scheduler of overlapping partitions
+__device__ __forceinline__ bool jq_exclusive(const JobQ& q) { return (q.flags & kJqExclusive) != 0; }
+__device__ __forceinline__ bool jq_has_gres(const JobQ& q) { return (q.flags & kJqHasGres) != 0; }
+__device__ __forceinline__ bool jq_general(const JobQ& q) { return (q.flags & kJqGeneral) != 0; }
+__device__ __forceinline__ uint32_t jq_gnames(const JobQ& q) { return (q.flags >> kJqNamesShift) & 0xffu; }
+__device__ __forceinline__ uint32_t jq_part(const JobQ& q) { return (q.flags >> kJqPartShift) & 7u; }
 
 struct PlaceDev {
   uint8_t* reason;
@@ -539,15 +550,15 @@ __global__ void k_build_jobq(PendingDev pd, const uint32_t* queue, const uint32_
   q.node_num = pd.node_num[j];
   q.alloc_off = pd.alloc_off[j];
   q.ntasks_per_node = t;
-  q.flags = (pd.exclusive[j] ? 1u : 0u) | (view_has_gres(q.req) ? 2u : 0u);
+  q.flags = (pd.exclusive[j] ? kJqExclusive : 0u) | (view_has_gres(q.req) ? kJqHasGres : 0u);
   q.ntpn_max = pd.ntasks_per_node_max[j];
   q.ntasks = pd.ntasks[j];
   q.vpart = vpart[j];
-  // partition inside a scheduler of overlapping partitions (bits 16-18)
-  if (q.vpart < cl_n_comp && part_cidx) q.flags |= (part_cidx[pd.partition[j]] & 7u) << 16;
+  // partition inside a scheduler of overlapping partitions
+  if (q.vpart < cl_n_comp && part_cidx) q.flags |= (part_cidx[pd.partition[j]] & 7u) << kJqPartShift;
   // anything but "exactly ntasks_per_node tasks on each of node_num nodes" takes the general
   // task distribution (JobScheduler.cpp:5193-5222, 5340-5361)
-  if (q.ntpn_max != t || (uint64_t)t * q.node_num != q.ntasks) q.flags |= 4u;
+  if (q.ntpn_max != t || (uint64_t)t * q.node_num != q.ntasks) q.flags |= kJqGeneral;
   q.spec8 = 0;
   for (uint32_t g = 0; g < CRANE_GRES_NAMES; ++g) {
     uint32_t typed = 0;
@@ -559,7 +570,7 @@ __global__ void k_build_jobq(PendingDev pd, const uint32_t* queue, const uint32_
     const uint32_t tot = field16(q.req.gtot, g);
     const uint32_t need = tot > typed ? tot : typed;
     q.name_need[g] = (uint8_t)(need > 255 ? 255 : need);
-    if (need) q.flags |= 1u << (8 + g);
+    if (need) q.flags |= 1u << (kJqNamesShift + g);
   }
   jobq[r] = q;
 }
@@ -686,7 +697,7 @@ __global__ void k_feas_bitmap(ClusterDev cl, PendingDev pd, const JobQ* jobq, co
     JobQ jq = jobq[r];
     uint32_t p = jq.vpart;
     if (part_owner && part_owner[p] != rank) continue;  // another GPU commits this scheduler
-    const uint32_t cidx = (jq.flags >> 16) & 7u;
+    const uint32_t cidx = jq_part(jq);
     uint32_t base = cl.part_base[p], mp = cl.part_base[p + 1] - base;
     const uint32_t row_words = (mp + 31) / 32;          // words beyond the job's own partition are never read
     uint32_t il = 0, ih = 0, el = 0, eh = 0;
