@@ -618,3 +618,135 @@ class Reservations:
     def as_c(self) -> ReservationsC:
         return ReservationsC(self.n, _ptr(self.start_time), _ptr(self.end_time), _ptr(self.node_off),
                              _ptr(self.node), _ptr(self.res))
+
+
+# ---------------------------------------------------------------------------
+# The step scheduler of running jobs (JobInCtld::SchedulePendingSteps)
+# ---------------------------------------------------------------------------
+class StepJobsC(C.Structure):
+    """crane_step_jobs_t"""
+    _fields_ = [("n_jobs", C.c_uint32), ("node_off", _p), ("node", _p), ("avail", _p), ("step_off", _p)]
+
+
+class StepsC(C.Structure):
+    """crane_steps_t"""
+    _fields_ = [("n", C.c_uint32), ("node_num", _p), ("ntasks", _p), ("ntasks_per_node_min", _p),
+                ("ntasks_per_node_max", _p), ("req_node", _p), ("req_task", _p), ("incl_off", _p),
+                ("incl_nodes", _p), ("excl_off", _p), ("excl_nodes", _p)]
+
+
+class StepPlacementsC(C.Structure):
+    """crane_step_placements_t"""
+    _fields_ = [("placed", _p), ("scheduled", _p), ("node_off", _p), ("alloc_node", _p), ("alloc_ntasks", _p),
+                ("alloc_res", _p), ("task_off", _p), ("task_node", _p), ("task_res", _p)]
+
+
+@dataclass
+class StepJobs:
+    """Running jobs with pending steps: their nodes, step_res_avail_ (one row per
+    (job, node), updated in place by the scheduler) and the CSR of their FIFO steps."""
+    node_off: np.ndarray
+    node: np.ndarray
+    avail: np.ndarray
+    step_off: np.ndarray
+
+    def __post_init__(self):
+        self.node_off = _arr(self.node_off, np.uint32)
+        n = len(self.node_off) - 1
+        self.node = _arr(self.node, np.uint32, int(self.node_off[-1]))
+        self.avail = _arr(self.avail, RES_IN_NODE, int(self.node_off[-1]))
+        self.step_off = _arr(self.step_off, np.uint32, n + 1)
+
+    @property
+    def n_jobs(self):
+        return len(self.node_off) - 1
+
+    def copy(self) -> "StepJobs":
+        return StepJobs(self.node_off.copy(), self.node.copy(), self.avail.copy(), self.step_off.copy())
+
+    def as_c(self) -> StepJobsC:
+        return StepJobsC(self.n_jobs, _ptr(self.node_off), _ptr(self.node), _ptr(self.avail), _ptr(self.step_off))
+
+
+@dataclass
+class Steps:
+    """The fields of CommonStepInCtld the step scheduler reads, one row per step."""
+    node_num: np.ndarray
+    ntasks: np.ndarray
+    ntasks_per_node_min: np.ndarray
+    ntasks_per_node_max: np.ndarray
+    req_node: np.ndarray
+    req_task: np.ndarray
+    incl_off: np.ndarray | None = None
+    incl_nodes: np.ndarray | None = None
+    excl_off: np.ndarray | None = None
+    excl_nodes: np.ndarray | None = None
+
+    def __post_init__(self):
+        n = len(self.node_num)
+        for f in ("node_num", "ntasks", "ntasks_per_node_min", "ntasks_per_node_max"):
+            setattr(self, f, _arr(getattr(self, f), np.uint32, n))
+        self.req_node = _arr(self.req_node, RES_VIEW, n)
+        self.req_task = _arr(self.req_task, RES_VIEW, n)
+        for k in ("incl", "excl"):
+            off = getattr(self, k + "_off")
+            if off is not None:
+                setattr(self, k + "_off", _arr(off, np.uint32, n + 1))
+                setattr(self, k + "_nodes", _arr(getattr(self, k + "_nodes"), np.uint32))
+
+    @property
+    def n(self):
+        return len(self.node_num)
+
+    def as_c(self) -> StepsC:
+        return StepsC(self.n, _ptr(self.node_num), _ptr(self.ntasks), _ptr(self.ntasks_per_node_min),
+                      _ptr(self.ntasks_per_node_max), _ptr(self.req_node), _ptr(self.req_task),
+                      _ptr(self.incl_off), _ptr(self.incl_nodes), _ptr(self.excl_off), _ptr(self.excl_nodes))
+
+
+@dataclass
+class StepPlacements:
+    """What SchedulePendingSteps writes: per job the steps placed at the head of its
+    queue, per step `scheduled`, node rows (node-index order) and task rows (task-id order)."""
+    placed: np.ndarray
+    scheduled: np.ndarray
+    node_off: np.ndarray
+    alloc_node: np.ndarray
+    alloc_ntasks: np.ndarray
+    alloc_res: np.ndarray
+    task_off: np.ndarray
+    task_node: np.ndarray
+    task_res: np.ndarray
+
+    @staticmethod
+    def for_steps(jobs: StepJobs, steps: Steps) -> "StepPlacements":
+        nr = int(steps.node_num.astype(np.int64).sum())
+        tr = int(steps.ntasks.astype(np.int64).sum())
+        z = np.zeros
+        return StepPlacements(z(jobs.n_jobs, np.uint32), z(steps.n, np.uint8), z(steps.n + 1, np.uint32),
+                              z(nr, np.uint32), z(nr, np.uint32), z(nr, RES_IN_NODE), z(steps.n + 1, np.uint32),
+                              z(tr, np.uint32), z(tr, RES_IN_NODE))
+
+    def as_c(self) -> StepPlacementsC:
+        return StepPlacementsC(*[_ptr(getattr(self, f)) for f in self.__dataclass_fields__])
+
+    def diff(self, other: "StepPlacements") -> list[str]:
+        """Field-by-field bit-exact comparison; returns mismatch descriptions."""
+        out = []
+        for f in self.__dataclass_fields__:
+            a, b = getattr(self, f), getattr(other, f)
+            if a.shape != b.shape:
+                out.append(f"{f}: shape {a.shape} vs {b.shape}")
+                continue
+            neq = a.view(np.uint8).reshape(len(a), -1) != b.view(np.uint8).reshape(len(b), -1)
+            bad = np.flatnonzero(neq.any(axis=1)) if len(a) else np.zeros(0, int)
+            if len(bad):
+                out.append(f"{f}: {len(bad)} mismatches, first at {bad[:5].tolist()}: {a[bad[0]]} vs {b[bad[0]]}")
+        return out
+
+    def digest(self) -> str:
+        import hashlib
+        h = hashlib.sha256()
+        for f in self.__dataclass_fields__:
+            h.update(np.ascontiguousarray(getattr(self, f)).tobytes())
+        return h.hexdigest()

@@ -497,3 +497,113 @@ void SchedulerAlgo::CheckAndMallocQosResource(const std::map<std::string, Qos>& 
 }
 
 }  // namespace crane_b200
+
+namespace crane_b200 {
+
+std::vector<uint32_t> SchedulerAlgo::SchedulePendingSteps(int64_t now, const std::vector<JobStepState*>& jobs,
+                                                          std::vector<std::vector<CommonStepInCtld*>>* scheduled_steps) {
+  Impl& m = *m_;
+  const uint32_t J = (uint32_t)jobs.size();
+  // ---- jobs: nodes of step_res_avail_ (index-ascending) + the live steps in FIFO order ----
+  std::vector<uint32_t> node_off(J + 1, 0), node, step_off(J + 1, 0);
+  std::vector<crane_res_in_node_t> avail;
+  std::vector<CommonStepInCtld*> live;
+  for (uint32_t j = 0; j < J; ++j) {
+    const JobStepState& js = *jobs[j];
+    std::vector<std::pair<uint32_t, const ResourceInNodeV3*>> nodes;
+    for (const auto& [id, res] : js.step_res_avail) {
+      auto it = m.node_index.find(id);
+      if (it == m.node_index.end()) throw std::runtime_error("step_res_avail_ node not in the cluster: " + id);
+      nodes.push_back({it->second, &res});
+    }
+    std::sort(nodes.begin(), nodes.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+    for (const auto& [idx, res] : nodes) {
+      node.push_back(idx);
+      avail.push_back(m.ToRow(idx, *res));
+    }
+    node_off[j + 1] = (uint32_t)node.size();
+    for (uint32_t id : js.pending_step_ids) {
+      auto it = js.steps.find(id);
+      if (it != js.steps.end()) live.push_back(it->second);  // GetStep() == nullptr: removed (:1883-1889)
+    }
+    step_off[j + 1] = (uint32_t)live.size();
+  }
+  const uint32_t S = (uint32_t)live.size();
+  std::vector<uint32_t> nn(S), nt(S), t0(S), t1(S), incl_off(S + 1, 0), incl, excl_off(S + 1, 0), excl;
+  std::vector<crane_res_view_t> vn(S), vt(S);
+  auto list_index = [&](const std::string& id) {
+    auto it = m.node_index.find(id);
+    return it == m.node_index.end() ? 0xFFFFFFFFu : it->second;  // a host the cluster does not know
+  };
+  for (uint32_t s = 0; s < S; ++s) {
+    const CommonStepInCtld& x = *live[s];
+    nn[s] = x.node_num;
+    nt[s] = x.ntasks;
+    t0[s] = x.ntasks_per_node_min;
+    t1[s] = x.ntasks_per_node_max;
+    vn[s] = m.ToView(x.req_node_res_view);
+    vt[s] = m.ToView(x.req_task_res_view);
+    for (const auto& id : x.included_nodes) incl.push_back(list_index(id));
+    incl_off[s + 1] = (uint32_t)incl.size();
+    for (const auto& id : x.excluded_nodes) {
+      const uint32_t n = list_index(id);
+      if (n != 0xFFFFFFFFu) excl.push_back(n);  // an unknown host excludes nothing
+    }
+    excl_off[s + 1] = (uint32_t)excl.size();
+  }
+  crane_step_jobs_t cj{J, node_off.data(), node.data(), avail.data(), step_off.data()};
+  crane_steps_t cs{S, nn.data(), nt.data(), t0.data(), t1.data(), vn.data(), vt.data(),
+                   incl_off.data(), incl.data(), excl_off.data(), excl.data()};
+  uint64_t nrows = 0, trows = 0;
+  for (uint32_t s = 0; s < S; ++s) { nrows += nn[s]; trows += nt[s]; }
+  std::vector<uint32_t> placed(J), o_noff(S + 1), o_node(nrows), o_ntasks(nrows), o_toff(S + 1), o_tnode(trows);
+  std::vector<uint8_t> sched(S);
+  std::vector<crane_res_in_node_t> o_res(nrows), o_tres(trows);
+  crane_step_placements_t out{placed.data(), sched.data(), o_noff.data(), o_node.data(), o_ntasks.data(),
+                              o_res.data(), o_toff.data(), o_tnode.data(), o_tres.data()};
+  int rc = crane_sched_schedule_steps(m.h, &cj, &cs, &out, nullptr);
+  if (rc != CRANE_OK) throw std::runtime_error(std::string("crane_sched_schedule_steps: ") + crane_sched_last_error(m.h));
+
+  // ---- write back ------------------------------------------------------------------
+  if (scheduled_steps) scheduled_steps->assign(J, {});
+  std::vector<uint32_t> popped(J, 0);
+  for (uint32_t j = 0; j < J; ++j) {
+    JobStepState& js = *jobs[j];
+    for (uint32_t k = node_off[j]; k < node_off[j + 1]; ++k)
+      js.step_res_avail[m.node_names[node[k]]] = m.FromRow(node[k], avail[k]);
+    uint32_t live_left = placed[j];
+    uint32_t s = step_off[j];
+    // the reference pops removed ids and scheduled steps off the front until a step blocks
+    while (!js.pending_step_ids.empty()) {
+      auto it = js.steps.find(js.pending_step_ids.front());
+      if (it != js.steps.end()) {
+        if (live_left == 0) break;
+        CommonStepInCtld& x = *it->second;
+        x.craned_task_map.clear();
+        x.task_res_map.clear();
+        x.allocated_res.clear();
+        x.craned_ids.clear();
+        for (uint32_t r = o_noff[s]; r < o_noff[s + 1]; ++r) {
+          const CranedId& id = m.node_names[o_node[r]];
+          x.craned_ids.push_back(id);
+          x.allocated_res.emplace(id, m.FromRow(o_node[r], o_res[r]));
+          x.craned_task_map[id];
+        }
+        for (uint32_t t = 0; t < nt[s]; ++t) {
+          const uint32_t r = o_toff[s] + t;
+          x.craned_task_map[m.node_names[o_tnode[r]]].insert(t);
+          x.task_res_map[t] = m.FromRow(o_tnode[r], o_tres[r]);
+        }
+        x.start_time = now;
+        if (scheduled_steps) (*scheduled_steps)[j].push_back(&x);
+        --live_left;
+        ++s;
+      }
+      js.pending_step_ids.pop_front();
+      ++popped[j];
+    }
+  }
+  return popped;
+}
+
+}  // namespace crane_b200

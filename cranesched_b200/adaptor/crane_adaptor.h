@@ -16,6 +16,7 @@
 #pragma once
 
 #include <cstdint>
+#include <deque>
 #include <list>
 #include <map>
 #include <memory>
@@ -156,6 +157,35 @@ struct QosUsage {
   std::map<std::string, MetaResource> qos;
 };
 
+// CommonStepInCtld (CtldPublicDefs.h:481-720): the fields JobInCtld::SchedulePendingSteps
+// reads (request) and writes (placement)
+struct CommonStepInCtld {
+  uint32_t step_id{0};
+  uint32_t node_num{1};
+  uint32_t ntasks{1};
+  uint32_t ntasks_per_node_min{1};
+  uint32_t ntasks_per_node_max{1};
+  ResourceView req_node_res_view;
+  ResourceView req_task_res_view;
+  std::unordered_set<std::string> included_nodes;
+  std::unordered_set<std::string> excluded_nodes;
+  // ---- written when the step is scheduled ---------------------------------
+  std::unordered_map<CranedId, std::set<uint32_t>> craned_task_map;
+  std::unordered_map<uint32_t, ResourceInNodeV3> task_res_map;
+  ResourceV3 allocated_res;
+  std::vector<CranedId> craned_ids;  // node-index ascending
+  int64_t start_time{0};
+};
+
+// The step state of a running JobInCtld (CtldPublicDefs.h:823-824, 991-1000):
+// pending_step_ids_ (a std::queue upstream), step_res_avail_, and GetStep() — an id
+// without an entry in `steps` is a step that was removed while queued.
+struct JobStepState {
+  std::deque<uint32_t> pending_step_ids;
+  ResourceV3 step_res_avail;
+  std::unordered_map<uint32_t, CommonStepInCtld*> steps;
+};
+
 class SchedulerAlgo {
  public:
   SchedulerAlgo(const PriorityConfig& prio, uint32_t scheduled_batch_size, int device = 0);
@@ -186,6 +216,17 @@ class SchedulerAlgo {
   // Call right after NodeSelect with the same pending_jobs.
   void CheckAndMallocQosResource(const std::map<std::string, Qos>& qos_table, QosUsage& usage,
                                  const std::vector<std::unique_ptr<PdJobInScheduler>>& pending_jobs);
+
+  // Replaces the JobInCtld::SchedulePendingSteps calls of StepScheduleThread_
+  // (JobScheduler.cpp:1646-1659; CtldPublicDefs.cpp:1877-1998) for all jobs at once.
+  // Per job, returns the reference's popped_count: the ids taken off the front of
+  // pending_step_ids — scheduled steps and removed ones — up to the first step that
+  // does not fit (removed ids behind it stay queued). Scheduled steps get
+  // craned_task_map, task_res_map, allocated_res, craned_ids and start_time = now, are
+  // appended to (*scheduled_steps)[j], and step_res_avail is updated. Status, the
+  // ia_meta callback, the DB and the RPC stay with the daemon. Call after SetCluster.
+  std::vector<uint32_t> SchedulePendingSteps(int64_t now, const std::vector<JobStepState*>& jobs,
+                                             std::vector<std::vector<CommonStepInCtld*>>* scheduled_steps);
 
  private:
   struct Impl;

@@ -29,6 +29,7 @@
 #include "sched_kernels.cuh"
 #include "commit_v2.cuh"
 #include "qos_kernels.cuh"
+#include "step_kernels.cuh"
 
 using namespace crane;
 
@@ -79,7 +80,7 @@ struct crane_sched {
   crane_sched_config_t cfg{};
   int device = 0;
   cudaStream_t stream = nullptr;
-  cudaEvent_t ev[10]{};  // 0-1 upload, 2-7 run / fetch, 8-9 qos filter
+  cudaEvent_t ev[12]{};  // 0-1 upload, 2-7 run / fetch, 8-9 qos filter, 10-11 step scheduler
   std::string err;
   crane_sched_timing_t timing{};
   size_t v2_budget = 0;       // dynamic shared memory k_commit2 may use
@@ -172,6 +173,11 @@ struct crane_sched {
   DBuf<uint8_t> d_q_valid;
   DBuf<crane_tres_limit_t> d_q_tres;
   DBuf<crane_meta_resource_t> d_q_user_usage, d_q_acct_usage, d_q_qos_usage;
+  // step scheduler (per call)
+  DBuf<uint32_t> d_st_u32;   // job node_off | node | step_off | step columns | lists | out offsets | placed | alloc_node | alloc_ntasks | task_node
+  DBuf<Row> d_st_rows;       // avail | alloc_res | task_res
+  DBuf<View> d_st_views;     // req_node | req_task
+  DBuf<uint8_t> d_st_sched;
 };
 
 namespace {
@@ -303,6 +309,7 @@ void crane_sched_destroy(crane_sched_t* h) {
   REL(d_out_res); REL(d_prof); REL(d_qos); REL(d_user); REL(d_q_u32); REL(d_q_chain_off); REL(d_q_chain);
   REL(d_q_i64); REL(d_q_valid); REL(d_part_owner); REL(d_part_list); REL(d_ntpn_max); REL(d_ntasks); REL(d_first_resv); REL(d_resv_start); REL(d_resv_end); REL(d_slot_resv);
   REL(d_rsv_off); REL(d_rsv_id); REL(d_dead); REL(d_erase_rows); REL(d_q_off); REL(d_sched_nparts); REL(d_part_comp); REL(d_part_cidx); REL(d_sched_owner); REL(d_slot_memb); REL(d_vpart); REL(d_pd_resv); REL(d_rsv_res); REL(d_q_tres); REL(d_q_user_usage); REL(d_q_acct_usage); REL(d_q_qos_usage);
+  REL(d_st_u32); REL(d_st_rows); REL(d_st_views); REL(d_st_sched);
 #undef REL
   for (auto& e : h->ev) cudaEventDestroy(e);
   cudaStreamDestroy(h->stream);
@@ -1297,6 +1304,133 @@ int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_
   CU(cudaStreamSynchronize(h->stream));
   h->timing.qos_ms = 0.f;
   if (N) cudaEventElapsedTime(&h->timing.qos_ms, h->ev[8], h->ev[9]);
+  return CRANE_OK;
+}
+
+int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, const crane_steps_t* st,
+                               crane_step_placements_t* out, float* device_ms) {
+  if (!h || !jb || !st || !out) return CRANE_EINVAL;
+  if (!h->have_cluster) return fail(h, CRANE_EINVAL, "schedule_steps: set_cluster first");
+  const uint32_t J = jb->n_jobs;
+  if (!jb->node_off || !jb->step_off) return fail(h, CRANE_EINVAL, "step jobs: null offsets");
+  if (jb->node_off[0] != 0 || jb->step_off[0] != 0) return fail(h, CRANE_EINVAL, "step jobs: offsets must start at 0");
+  for (uint32_t j = 0; j < J; ++j) {
+    if (jb->node_off[j + 1] < jb->node_off[j] || jb->step_off[j + 1] < jb->step_off[j])
+      return fail(h, CRANE_EINVAL, "step jobs: offsets are not monotonic");
+  }
+  const uint32_t E = jb->node_off[J], S = jb->step_off[J];
+  if (st->n != S) return fail(h, CRANE_EINVAL, "steps: n (%u) != step_off[n_jobs] (%u)", st->n, S);
+  if (E && (!jb->node || !jb->avail)) return fail(h, CRANE_EINVAL, "step jobs: null node table");
+  for (uint32_t j = 0; j < J; ++j)
+    for (uint32_t k = jb->node_off[j]; k < jb->node_off[j + 1]; ++k) {
+      if (jb->node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "step jobs[%u]: node %u out of range", j, jb->node[k]);
+      if (k > jb->node_off[j] && jb->node[k] <= jb->node[k - 1])
+        return fail(h, CRANE_EINVAL, "step jobs[%u]: nodes must be ascending and distinct", j);
+    }
+  if (S && (!st->node_num || !st->ntasks || !st->ntasks_per_node_min || !st->ntasks_per_node_max || !st->req_node ||
+            !st->req_task))
+    return fail(h, CRANE_EINVAL, "steps: null column");
+  uint64_t nrows = 0, trows = 0;
+  for (uint32_t s = 0; s < S; ++s) {
+    const uint32_t nn = st->node_num[s], nt = st->ntasks[s], t0 = st->ntasks_per_node_min[s], t1 = st->ntasks_per_node_max[s];
+    if (nn == 0) return fail(h, CRANE_EINVAL, "steps[%u]: node_num == 0", s);
+    if (nt < nn) return fail(h, CRANE_EINVAL, "steps[%u]: ntasks < node_num", s);
+    if (t0 > t1) return fail(h, CRANE_EINVAL, "steps[%u]: ntasks_per_node_min > ntasks_per_node_max", s);
+    if (nn >= (uint32_t)kStepHeapMax) return fail(h, CRANE_ENOSYS, "steps[%u]: node_num above %d", s, kStepHeapMax - 1);
+    // (a node could then be picked for no task; the reference hands it ntasks - node_num + 1 unchecked allocations)
+    if (t0 == 0) return fail(h, CRANE_ENOSYS, "steps[%u]: ntasks_per_node_min == 0", s);
+    if (st->req_node[s].cpu_raw < 0 || st->req_task[s].cpu_raw < 0) return fail(h, CRANE_EINVAL, "steps[%u]: negative cpu request", s);
+    nrows += nn;
+    trows += nt;
+  }
+  if (nrows > 0xfffffff0ull || trows > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "steps: too many node / task rows");
+  for (int l = 0; l < 2; ++l) {
+    const uint32_t* off = l ? st->excl_off : st->incl_off;
+    const uint32_t* nodes = l ? st->excl_nodes : st->incl_nodes;
+    if (!off) continue;
+    if (off[0] != 0) return fail(h, CRANE_EINVAL, "steps: node list offsets must start at 0");
+    for (uint32_t s = 0; s < S; ++s)
+      if (off[s + 1] < off[s]) return fail(h, CRANE_EINVAL, "steps[%u]: node list offsets are not monotonic", s);
+    if (off[S] && !nodes) return fail(h, CRANE_EINVAL, "steps: node list CSR without node array");
+    for (uint32_t k = 0; k < off[S]; ++k)
+      if (nodes[k] >= h->n_nodes && nodes[k] != 0xFFFFFFFFu) return fail(h, CRANE_EINVAL, "steps: listed node out of range");
+  }
+  if ((J && !out->placed) || (S && (!out->scheduled || !out->node_off || !out->task_off)) || !out->node_off || !out->task_off ||
+      (nrows && (!out->alloc_node || !out->alloc_ntasks || !out->alloc_res)) || (trows && (!out->task_node || !out->task_res)))
+    return fail(h, CRANE_EINVAL, "step placements: null column");
+  CU(cudaSetDevice(h->device));
+  (void)cudaGetLastError();
+  cudaStream_t sm = h->stream;
+
+  // one u32 table, one row table, one view table: three copies in, five out
+  std::vector<uint32_t> u;
+  u.reserve((size_t)3 * J + E + 8 * (size_t)S + 8);
+  auto put = [&](const uint32_t* p, size_t n) { size_t at = u.size(); u.insert(u.end(), p, p + n); return at; };
+  const size_t o_noff = put(jb->node_off, (size_t)J + 1);
+  const size_t o_node = put(jb->node, E);
+  const size_t o_soff = put(jb->step_off, (size_t)J + 1);
+  const size_t o_nn = put(st->node_num, S), o_nt = put(st->ntasks, S);
+  const size_t o_t0 = put(st->ntasks_per_node_min, S), o_t1 = put(st->ntasks_per_node_max, S);
+  size_t o_io = 0, o_in = 0, o_eo = 0, o_en = 0;
+  if (st->incl_off) { o_io = put(st->incl_off, (size_t)S + 1); o_in = put(st->incl_nodes, st->incl_off[S]); }
+  if (st->excl_off) { o_eo = put(st->excl_off, (size_t)S + 1); o_en = put(st->excl_nodes, st->excl_off[S]); }
+  out->node_off[0] = 0;
+  out->task_off[0] = 0;
+  for (uint32_t s = 0; s < S; ++s) {
+    out->node_off[s + 1] = out->node_off[s] + st->node_num[s];
+    out->task_off[s + 1] = out->task_off[s] + st->ntasks[s];
+  }
+  const size_t o_ooff = put(out->node_off, (size_t)S + 1), o_toff = put(out->task_off, (size_t)S + 1);
+  const size_t n_in = u.size();
+  const size_t o_placed = n_in, o_anode = o_placed + J, o_antasks = o_anode + nrows, o_tnode = o_antasks + nrows;
+  const size_t n_u32 = o_tnode + trows;
+  CU(h->d_st_u32.ensure(std::max<size_t>(n_u32, 1)));
+  CU(h->d_st_rows.ensure(std::max<size_t>(E + nrows + trows, 1)));
+  CU(h->d_st_views.ensure(std::max<size_t>(2 * (size_t)S, 1)));
+  CU(h->d_st_sched.ensure(std::max<size_t>(S, 1)));
+  uint32_t* du = h->d_st_u32.p;
+  Row* dr = h->d_st_rows.p;
+  View* dv = h->d_st_views.p;
+  CU(cudaMemcpyAsync(du, u.data(), n_in * sizeof(uint32_t), cudaMemcpyHostToDevice, sm));
+  if (n_u32 > n_in) CU(cudaMemsetAsync(du + n_in, 0, (n_u32 - n_in) * sizeof(uint32_t), sm));
+  if (E) CU(cudaMemcpyAsync(dr, jb->avail, E * sizeof(Row), cudaMemcpyHostToDevice, sm));
+  if (nrows + trows) CU(cudaMemsetAsync(dr + E, 0, (nrows + trows) * sizeof(Row), sm));
+  if (S) {
+    CU(cudaMemcpyAsync(dv, st->req_node, S * sizeof(View), cudaMemcpyHostToDevice, sm));
+    CU(cudaMemcpyAsync(dv + S, st->req_task, S * sizeof(View), cudaMemcpyHostToDevice, sm));
+    CU(cudaMemsetAsync(h->d_st_sched.p, 0, S, sm));
+  }
+  StepJobsDev dj{J, du + o_noff, du + o_node, dr, du + o_soff};
+  StepsDev ds{du + o_nn, du + o_nt, du + o_t0, du + o_t1, dv, dv + S,
+              st->incl_off ? du + o_io : nullptr, du + o_in, st->excl_off ? du + o_eo : nullptr, du + o_en};
+  StepOutDev dout{du + o_placed, h->d_st_sched.p, du + o_ooff, du + o_anode, du + o_antasks, dr + E,
+                  du + o_toff, du + o_tnode, dr + E + nrows};
+  CU(cudaEventRecord(h->ev[10], sm));
+  if (J) {
+    const uint32_t grid = std::min<uint32_t>((J + kStepWarps - 1) / kStepWarps, 16 * h->n_sm);
+    CRANE_LAUNCH(k_steps, grid, 32 * kStepWarps, 0, sm, dj, ds, dout, (uint32_t)h->dict_slot);
+    CU(cudaGetLastError());
+  }
+  CU(cudaEventRecord(h->ev[11], sm));
+  if (J) CU(cudaMemcpyAsync(out->placed, du + o_placed, J * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+  if (S) CU(cudaMemcpyAsync(out->scheduled, h->d_st_sched.p, S, cudaMemcpyDeviceToHost, sm));
+  if (nrows) {
+    CU(cudaMemcpyAsync(out->alloc_node, du + o_anode, nrows * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->alloc_ntasks, du + o_antasks, nrows * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->alloc_res, dr + E, nrows * sizeof(Row), cudaMemcpyDeviceToHost, sm));
+  }
+  if (trows) {
+    CU(cudaMemcpyAsync(out->task_node, du + o_tnode, trows * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->task_res, dr + E + nrows, trows * sizeof(Row), cudaMemcpyDeviceToHost, sm));
+  }
+  if (E) CU(cudaMemcpyAsync(jb->avail, dr, E * sizeof(Row), cudaMemcpyDeviceToHost, sm));
+  CU(cudaStreamSynchronize(sm));
+  CU(cudaGetLastError());
+  if (device_ms) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, h->ev[10], h->ev[11]);
+    *device_ms = ms;
+  }
   return CRANE_OK;
 }
 

@@ -81,6 +81,9 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.crane_sched_debug_bitmap.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, P(C.c_uint32), P(C.c_uint32)]
     lib.crane_sched_debug_profile.restype = C.c_int
     lib.crane_sched_debug_profile.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.crane_sched_schedule_steps.restype = C.c_int
+    lib.crane_sched_schedule_steps.argtypes = [C.c_void_p, P(abi.StepJobsC), P(abi.StepsC), P(abi.StepPlacementsC),
+                                               P(C.c_float)]
     _libs[path] = lib
     return lib
 
@@ -90,7 +93,7 @@ EXPORTS = ("crane_sched_create", "crane_sched_destroy", "crane_sched_last_error"
            "crane_sched_set_running", "crane_sched_pending_rows",
            "crane_sched_run", "crane_sched_fetch", "crane_sched_sync", "crane_sched_get_timing",
            "crane_sched_qos_filter", "crane_sched_set_shard", "crane_sched_device_placements",
-           "crane_sched_debug_bitmap", "crane_sched_debug_profile")
+           "crane_sched_debug_bitmap", "crane_sched_debug_profile", "crane_sched_schedule_steps")
 
 
 class GpuScheduler:
@@ -197,6 +200,17 @@ class GpuScheduler:
         c_q = qos.as_c()
         self._check(self._lib.crane_sched_qos_filter(self._h, C.byref(c_q), reason.ctypes.data))
         return reason
+
+    # --- the step scheduler of running jobs ------------------------------------------
+    def schedule_steps(self, jobs: abi.StepJobs, steps: abi.Steps,
+                       out: abi.StepPlacements | None = None) -> tuple[abi.StepPlacements, float]:
+        """JobInCtld::SchedulePendingSteps for every job of `jobs` (CtldPublicDefs.cpp:1877-1998),
+        after set_cluster (its gres dictionary). jobs.avail is updated in place.
+        Returns (placements, device ms of the step kernel)."""
+        out = out if out is not None else abi.StepPlacements.for_steps(jobs, steps)
+        c_j, c_s, c_o, ms = jobs.as_c(), steps.as_c(), out.as_c(), C.c_float(0.0)
+        self._check(self._lib.crane_sched_schedule_steps(self._h, C.byref(c_j), C.byref(c_s), C.byref(c_o), C.byref(ms)))
+        return out, ms.value
 
     def timing(self) -> dict:
         t = abi.TimingC()

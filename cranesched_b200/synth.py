@@ -597,3 +597,114 @@ def random_qos(seed, cluster, pend, tight=1.0, n_parents=4, invalid_frac=0.1):
 
 
 CONFIGS = {1: config1, 2: config2, 3: config3, 4: config4, 5: config5}
+
+
+# ---------------------------------------------------------------------------
+# Steps of running jobs (JobInCtld::SchedulePendingSteps): the jobs a NodeSelect
+# pass starts now become running jobs whose step_res_avail_ is their allocation
+# (JobScheduler.cpp:1277), each with a FIFO queue of srun / crun steps.
+# ---------------------------------------------------------------------------
+def started_jobs(pending: Pending, placements) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """(node_off, node, avail) of the jobs `placements` starts now, in job-id order."""
+    started = np.flatnonzero(placements.reason == 0)
+    nn = pending.node_num[started].astype(np.int64)
+    node_off = np.zeros(len(started) + 1, np.uint32)
+    node_off[1:] = np.cumsum(nn)
+    rows = (np.repeat(placements.alloc_off[started].astype(np.int64), nn)
+            + np.arange(int(nn.sum())) - np.repeat(node_off[:-1].astype(np.int64), nn))
+    return node_off, placements.alloc_node[rows].copy(), placements.alloc_res[rows].copy()
+
+
+def _step_ntpn(ntasks, nn, umin, umax):
+    """AcquireStepAttributes' ntasks_per_node bounds (JobScheduler.cpp:6410-6424)."""
+    dist_max = ntasks - nn + 1
+    tmax = dist_max if umax == 0 else min(umax, dist_max)
+    tmin = max(umin, ntasks - (nn - 1) * tmax, 1)
+    tmax = min(tmax, ntasks - (nn - 1) * tmin)
+    return tmin, tmax
+
+
+def step_case(seed, select, base=None, max_steps=6, one_type_per_name=False, **case_kw):
+    """(cluster, StepJobs, Steps) drawn over the jobs a NodeSelect case starts now.
+
+    select(cfg, cluster, running, pending, now) -> Placements runs the NodeSelect pass
+    (the GPU path or a CPU restatement); base is that case (default: random_case(seed,
+    ntpn_range=True, one_type_per_name=..., **case_kw)). Every job gets 0..max_steps
+    FIFO steps: ntasks_per_node ranges, include / exclude lists (with unknown hosts and
+    nodes outside the job), fractional and integer cpus, typed and untyped gres on the
+    node or the task request, steps that take the whole allocation, steps that cannot
+    fit (so later steps that would fit stay pending), and homogeneous requests whose
+    equal task counts tie in the heap."""
+    from .abi import StepJobs, Steps
+    if base is None:
+        base = random_case(seed, ntpn_range=True, one_type_per_name=one_type_per_name, **case_kw)
+    cfg, cluster, running, pending, now = base
+    node_off, node, avail = started_jobs(pending, select(cfg, cluster, running, pending, now))
+    rng = np.random.Generator(np.random.PCG64(seed ^ 0x57E9))
+    names = np.array(list(cluster.gres_entry_name) + [0] * (GRES_ENTRIES - cluster.n_gres_entries))
+    n_jobs = len(node_off) - 1
+    cols = {k: [] for k in ("node_num", "ntasks", "tmin", "tmax")}
+    req_node, req_task, incl, excl = [], [], [[0], []], [[0], []]
+    step_off = [0]
+    n_steps = rng.integers(0, max_steps + 1, n_jobs)
+    for j in range(n_jobs):
+        k0, k1 = int(node_off[j]), int(node_off[j + 1])
+        nk = k1 - k0
+        a = avail[k0:k1]
+        cpu_min, mem_min = int(a["cpu_raw"].min()), int(a["mem"].min())
+        gres_any = np.bitwise_or.reduce(a["gres"], axis=0) if nk else np.zeros(GRES_ENTRIES, np.uint16)
+        ents = [e for e in range(cluster.n_gres_entries) if gres_any[e]]
+        for _ in range(int(n_steps[j])):
+            vn, vt = np.zeros((), RES_VIEW), np.zeros((), RES_VIEW)
+            kind = rng.random()
+            if kind < 0.12:  # the whole allocation: one task per node, everything the smallest node holds
+                nn, ntasks, tmin, tmax = nk, nk, 1, 1
+                vt["cpu_raw"], vt["mem"], vt["mem_sw"] = cpu_min, mem_min, mem_min
+                for e in ents:
+                    cnt = min(bin(int(x)).count("1") for x in a["gres"][:, e])
+                    if cnt:
+                        vt["gres_spec"][e] = cnt
+                        vt["gres_total"][names[e]] += cnt
+            elif kind < 0.22:  # does not fit: blocks this job's queue
+                nn = min(nk + int(rng.integers(0, 2)), 127)
+                ntasks, tmin, tmax = nn, 1, 1
+                vt["cpu_raw"] = cpu_min + 256 if nn == nk else 64
+            else:
+                nn = int(rng.integers(1, nk + 1))
+                ntasks = nn * int(rng.choice([1, 1, 2, 3]))
+                if rng.random() < 0.5:
+                    ntasks += int(rng.integers(0, nn + 1))
+                tmin, tmax = _step_ntpn(ntasks, nn, int(rng.choice([1, 1, 2])), int(rng.choice([0, 0, 1, 2, 4])))
+                if tmin > tmax:
+                    ntasks, tmin, tmax = nn, 1, 1
+                vt["cpu_raw"] = int(rng.choice([64, 128, 384, 256, 256, 512, 1024]))
+                mem = int(rng.choice([0, 256 << 20, 1 << 30]))
+                vt["mem"], vt["mem_sw"] = mem, mem
+                if rng.random() < 0.2:
+                    vn["mem"] = vn["mem_sw"] = int(rng.choice([256 << 20, 1 << 30]))
+                if ents and rng.random() < 0.35:
+                    e = int(rng.choice(ents))
+                    v = vn if rng.random() < 0.5 else vt
+                    v["gres_total"][names[e]] += 1
+                    if rng.random() < 0.5:
+                        v["gres_spec"][e] += 1
+            if rng.random() < 0.12:  # include list: a subset of the job's nodes, maybe an unknown host / outsider
+                sub = sorted(rng.choice(node[k0:k1], int(rng.integers(1, nk + 1)), replace=False).tolist())
+                if rng.random() < 0.3:
+                    sub.append(0xFFFFFFFF if rng.random() < 0.5 else int(rng.integers(0, cluster.n_nodes)))
+                incl[1] += sub
+            incl[0].append(len(incl[1]))
+            if rng.random() < 0.12:
+                excl[1] += sorted(rng.choice(node[k0:k1], int(rng.integers(1, nk + 1)), replace=False).tolist())
+            excl[0].append(len(excl[1]))
+            for k, v in zip(cols, (nn, ntasks, tmin, tmax)):
+                cols[k].append(v)
+            req_node.append(vn)
+            req_task.append(vt)
+        step_off.append(len(cols["node_num"]))
+    jobs = StepJobs(node_off, node, avail, np.array(step_off, np.uint32))
+    steps = Steps(cols["node_num"], cols["ntasks"], cols["tmin"], cols["tmax"],
+                  np.array(req_node, RES_VIEW).reshape(-1), np.array(req_task, RES_VIEW).reshape(-1),
+                  np.array(incl[0], np.uint32), np.array(incl[1], np.uint32),
+                  np.array(excl[0], np.uint32), np.array(excl[1], np.uint32))
+    return cluster, jobs, steps

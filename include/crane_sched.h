@@ -388,6 +388,70 @@ typedef struct crane_qos_table {
  * "QosResourceLimit" (entry missing from a map) cannot occur. */
 int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qos, uint8_t* reason);
 
+/* ---- the step scheduler of running jobs ------------------------------------ */
+/* Running jobs with pending steps (srun / crun steps inside an allocation): the
+ * job's nodes, its step_res_avail_ (JobInCtld, seeded from the job's allocation
+ * at start, JobScheduler.cpp:1277) and its pending_step_ids_ queue. */
+typedef struct crane_step_jobs {
+  uint32_t n_jobs;
+  const uint32_t* node_off;   /* [n_jobs+1] CSR over (job, node) pairs          */
+  const uint32_t* node;       /* node index, ascending and distinct in a job    */
+  crane_res_in_node_t* avail; /* [node_off[n_jobs]] step_res_avail_ of the job on
+                                 that node; read and written in place          */
+  const uint32_t* step_off;   /* [n_jobs+1] the job's pending steps, FIFO, are the
+                                 rows [step_off[j], step_off[j+1]) of the steps */
+} crane_step_jobs_t;
+
+/* The fields of CommonStepInCtld the step scheduler reads, one row per pending
+ * step (conventions of crane_pending_t). ntasks_per_node_{min,max} as
+ * AcquireStepAttributes leaves them (JobScheduler.cpp:6410-6433). */
+typedef struct crane_steps {
+  uint32_t n;                        /* == step_off[n_jobs]                      */
+  const uint32_t* node_num;          /* 1 .. 127                                 */
+  const uint32_t* ntasks;            /* >= node_num                              */
+  const uint32_t* ntasks_per_node_min;  /* >= 1                                  */
+  const uint32_t* ntasks_per_node_max;
+  const crane_res_view_t* req_node;  /* req_node_res_view                        */
+  const crane_res_view_t* req_task;  /* req_task_res_view                        */
+  const uint32_t* incl_off;  /* [n+1] CSR of included_nodes, or NULL; 0xFFFFFFFF
+                                stands for a host unknown to the cluster         */
+  const uint32_t* incl_nodes;
+  const uint32_t* excl_off;  /* [n+1] CSR of excluded_nodes, or NULL            */
+  const uint32_t* excl_nodes;
+} crane_steps_t;
+
+/* What SchedulePendingSteps writes. Caller-owned, pre-sized. Step s owns node rows
+ * [node_off[s], node_off[s] + node_num[s]) in node-index order (node, tasks on it,
+ * its allocated_res: the node allocation plus its task allocations) and task rows
+ * [task_off[s], task_off[s] + ntasks[s]) in task-id order (node of the task and
+ * task_res_map[task id]); both offsets are exclusive prefix sums written by the
+ * callee. Rows of a step that was not scheduled are zero. */
+typedef struct crane_step_placements {
+  uint32_t* placed;        /* [n_jobs] steps placed at the head of the job's queue */
+  uint8_t* scheduled;      /* [n] 1 = scheduled now                             */
+  uint32_t* node_off;      /* [n+1]                                             */
+  uint32_t* alloc_node;    /* [sum node_num]                                    */
+  uint32_t* alloc_ntasks;  /* [sum node_num] craned_task_map[node].size()       */
+  crane_res_in_node_t* alloc_res; /* [sum node_num]                             */
+  uint32_t* task_off;      /* [n+1]                                             */
+  uint32_t* task_node;     /* [sum ntasks]                                      */
+  crane_res_in_node_t* task_res;  /* [sum ntasks]                               */
+} crane_step_placements_t;
+
+/* Replaces: the JobInCtld::SchedulePendingSteps calls of the step scheduler thread
+ * (CtldPublicDefs.cpp:1877-1998; JobScheduler.cpp:1637-1665), for every job at
+ * once; blocking. Each job takes its steps in FIFO order; a step that does not fit
+ * blocks every later step of its job. Nodes are walked in node-index order (the
+ * reference walks an unordered_map). Uses the gres dictionary of
+ * crane_sched_set_cluster and no NodeSelect state. *device_ms (optional) receives
+ * the CUDA-event time of the step kernel. CRANE_EINVAL for a node out of range or
+ * repeated / unordered within a job, node_num == 0, ntasks < node_num or
+ * ntasks_per_node_min > _max; CRANE_ENOSYS for node_num > 127 or
+ * ntasks_per_node_min == 0. */
+int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jobs,
+                               const crane_steps_t* steps, crane_step_placements_t* out,
+                               float* device_ms);
+
 /* Capability bitmap of the last run (the jobs x nodes feasibility bitmap):
  * bit (rank r, local node q) set iff the r-th job in priority order can run
  * on the q-th node of its partition by total resources and node lists
