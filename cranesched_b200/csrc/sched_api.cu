@@ -35,10 +35,17 @@ using namespace crane;
 
 namespace {
 
+// A device buffer that frees itself (with the handle's device current, see ~crane_sched)
 template <class T>
 struct DBuf {
   T* p = nullptr;
   size_t cap = 0;
+  DBuf() = default;
+  DBuf(const DBuf&) = delete;
+  DBuf& operator=(const DBuf&) = delete;
+  ~DBuf() {
+    if (p) cudaFree(p);
+  }
   cudaError_t ensure(size_t n) {
     if (n <= cap) return cudaSuccess;
     if (p) cudaFree(p);
@@ -66,13 +73,24 @@ struct DBuf {
     cap = want;
     return e;
   }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-  }
 };
 
+// How far a handle has got; each stage needs every earlier one. A call that replaces
+// the tables of a stage lowers the handle to the stage before it.
+enum Stage { kNone, kCluster, kUploaded, kRan };
+
+// The handle's CUDA events
+enum Ev {
+  kEvH2dBegin, kEvH2dEnd,                                                  // crane_sched_upload
+  kEvRunBegin, kEvInitEnd, kEvPrioEnd, kEvFeasEnd, kEvRunEnd, kEvD2hEnd,  // run, fetch
+  kEvQosBegin, kEvQosEnd,                                                  // qos_filter
+  kEvStepsBegin, kEvStepsEnd,                                              // schedule_steps
+  kNumEv
+};
+
+// c_dicts[] slots in use, per device
+std::mutex g_slot_mu;
+uint32_t g_slots_used[64] = {0};
 
 }  // namespace
 
@@ -80,16 +98,16 @@ struct crane_sched {
   crane_sched_config_t cfg{};
   int device = 0;
   cudaStream_t stream = nullptr;
-  cudaEvent_t ev[12]{};  // 0-1 upload, 2-7 run / fetch, 8-9 qos filter, 10-11 step scheduler
+  cudaEvent_t ev[kNumEv]{};
   std::string err;
   crane_sched_timing_t timing{};
   size_t v2_budget = 0;       // dynamic shared memory k_commit2 may use
   uint32_t n_sm = 0;          // SMs of the device: grid caps of the grid-stride kernels
-  bool h2d_timed = false;     // ev[0], ev[1] were recorded (crane_sched_upload)
+  bool h2d_timed = false;     // kEvH2dBegin, kEvH2dEnd were recorded (crane_sched_upload)
   uint32_t v2_ring = 0;
+  Stage stage = kNone;
 
   // cluster (host copies)
-  bool have_cluster = false;
   uint32_t n_nodes = 0, n_parts = 0, n_slots = 0, max_part_slots = 0, words_per_row = 0;
   uint32_t n_vparts = 0, n_resv = 0;  // schedulers = groups of overlapping partitions + reservations
   uint32_t n_comp = 0, max_comp_parts = 1;
@@ -160,7 +178,6 @@ struct crane_sched {
   DBuf<int64_t> d_out_start, d_out_end;
   DBuf<uint32_t> d_out_nalloc, d_out_node, d_out_ntasks;
   DBuf<Row> d_out_res;
-  bool uploaded = false, ran = false;
   int dict_slot = -1;  // this handle's entry of c_dicts[] on its device
   // one queue over several GPUs
   uint32_t shard_rank = 0, shard_n = 1;
@@ -178,13 +195,22 @@ struct crane_sched {
   DBuf<Row> d_st_rows;       // avail | alloc_res | task_res
   DBuf<View> d_st_views;     // req_node | req_task
   DBuf<uint8_t> d_st_sched;
+
+  // the buffers free themselves after this, on the handle's device
+  ~crane_sched() {
+    cudaSetDevice(device);
+    if (stream) cudaStreamSynchronize(stream);
+    for (auto& e : ev)
+      if (e) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
+    if (dict_slot >= 0) {
+      std::lock_guard<std::mutex> lk(g_slot_mu);
+      g_slots_used[device] &= ~(1u << dict_slot);
+    }
+  }
 };
 
 namespace {
-
-// c_dicts[] slots in use, per device
-std::mutex g_slot_mu;
-uint32_t g_slots_used[64] = {0};
 
 int fail(crane_sched* h, int code, const char* fmt, ...) {
   char buf[512];
@@ -203,17 +229,61 @@ int fail(crane_sched* h, int code, const char* fmt, ...) {
       return fail(h, e__ == 2 ? CRANE_ENOMEM : CRANE_ECUDA, "%s failed: %s", #call, cudaGetErrorString(e__)); \
   } while (0)
 
+#define TRY(call)                        \
+  do {                                   \
+    int rc__ = (call);                   \
+    if (rc__ != CRANE_OK) return rc__;   \
+  } while (0)
+
+// "<call>: <step> first" unless the handle has reached `want`
+int require(crane_sched* h, Stage want, const char* call) {
+  static const char* const step[] = {"", "set_cluster", "upload", "run"};
+  return h->stage >= want ? CRANE_OK : fail(h, CRANE_EINVAL, "%s: %s first", call, step[want]);
+}
+
+void lower_stage(crane_sched* h, Stage s) { h->stage = std::min(h->stage, s); }
+
+// The offsets of a CSR table of n rows: present, off[0] == 0, non-decreasing
+int check_offsets(crane_sched* h, const char* what, const uint32_t* off, uint32_t n) {
+  if (!off) return fail(h, CRANE_EINVAL, "%s: null offsets", what);
+  if (off[0] != 0) return fail(h, CRANE_EINVAL, "%s: offsets must start at 0", what);
+  for (uint32_t i = 0; i < n; ++i)
+    if (off[i + 1] < off[i]) return fail(h, CRANE_EINVAL, "%s[%u]: offsets are not monotonic", what, i);
+  return CRANE_OK;
+}
+
+// An include / exclude list CSR of n rows: its offsets, and every entry a node index
+// or 0xFFFFFFFF, a host the cluster does not know
+int check_node_list(crane_sched* h, const char* what, const uint32_t* off, const uint32_t* nodes, uint32_t n) {
+  TRY(check_offsets(h, what, off, n));
+  if (off[n] && !nodes) return fail(h, CRANE_EINVAL, "%s: node list CSR without node array", what);
+  for (uint32_t k = 0; k < off[n]; ++k)
+    if (nodes[k] >= h->n_nodes && nodes[k] != 0xFFFFFFFFu) return fail(h, CRANE_EINVAL, "%s: listed node out of range", what);
+  return CRANE_OK;
+}
+
+float elapsed_ms(const crane_sched* h, Ev from, Ev to) {
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, h->ev[from], h->ev[to]);
+  return ms;
+}
+
+// The phase times of the last run (its events have completed)
+void read_run_times(crane_sched* h) {
+  h->timing.init_ms = elapsed_ms(h, kEvRunBegin, kEvInitEnd);
+  h->timing.priority_ms = elapsed_ms(h, kEvInitEnd, kEvPrioEnd);
+  h->timing.feas_ms = elapsed_ms(h, kEvPrioEnd, kEvFeasEnd);
+  h->timing.commit_ms = elapsed_ms(h, kEvFeasEnd, kEvRunEnd);
+  h->timing.total_ms = elapsed_ms(h, kEvRunBegin, kEvRunEnd);
+}
+
 template <class T>
 int h2d(crane_sched* h, DBuf<T>& dst, const T* src, size_t n) {
   CU(dst.ensure(n ? n : 1));
   if (n) CU(cudaMemcpyAsync(dst.p, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream));
   return CRANE_OK;
 }
-#define H2D(buf, src, n)                      \
-  do {                                        \
-    int rc__ = h2d(h, buf, src, (size_t)(n)); \
-    if (rc__ != CRANE_OK) return rc__;        \
-  } while (0)
+#define H2D(buf, src, n) TRY(h2d(h, buf, src, (size_t)(n)))
 
 // stable LSD radix sort over bits [0, nbits) of d_keys_a with payload
 // d_vals_a; result pointers returned in keys/vals.
@@ -263,7 +333,6 @@ int crane_sched_create(const crane_sched_config_t* cfg, int device, crane_sched_
   h->device = device;
   h->dict_slot = slot;
   if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
-    { std::lock_guard<std::mutex> lk(g_slot_mu); g_slots_used[device] &= ~(1u << slot); }
     delete h;
     return CRANE_ENODEV;
   }
@@ -271,7 +340,7 @@ int crane_sched_create(const crane_sched_config_t* cfg, int device, crane_sched_
   int n_sm = 0, smem_optin = 0;
   if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device) != cudaSuccess ||
       cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess || n_sm <= 0) {
-    crane_sched_destroy(h);
+    delete h;
     return CRANE_ENODEV;
   }
   h->n_sm = (uint32_t)n_sm;
@@ -291,31 +360,7 @@ int crane_sched_create(const crane_sched_config_t* cfg, int device, crane_sched_
   return CRANE_OK;
 }
 
-void crane_sched_destroy(crane_sched_t* h) {
-  if (!h) return;
-  cudaSetDevice(h->device);
-  cudaStreamSynchronize(h->stream);
-#define REL(b) h->b.release()
-  REL(d_part_base); REL(d_slot_node); REL(d_node_slot); REL(d_slot_total); REL(d_tl_n); REL(d_tl_ent);
-  REL(d_avail0); REL(d_class_rows); REL(d_slot_class); REL(d_cost0); REL(d_skip); REL(d_partition);
-  REL(d_node_num); REL(d_ntpn); REL(d_part_prio); REL(d_qos_prio); REL(d_account); REL(d_alloc_off);
-  REL(d_time_limit); REL(d_submit); REL(d_exclusive); REL(d_mandated); REL(d_req_node); REL(d_req_task);
-  REL(d_req_total); REL(d_incl_off); REL(d_incl_nodes); REL(d_excl_off); REL(d_excl_nodes); REL(d_rn_start);
-  REL(d_rn_end); REL(d_rn_cpu); REL(d_rn_slot_end); REL(d_rn_node_num); REL(d_rn_part_prio); REL(d_rn_qos_prio);
-  REL(d_rn_account); REL(d_rn_slot_off); REL(d_rn_acc_off); REL(d_rn_acc_job); REL(d_rn_mem); REL(d_rn_slot_res);
-  REL(d_acc_present); REL(d_bounds); REL(d_acc_service); REL(d_prio); REL(d_keys_a); REL(d_keys_b); REL(d_vals_a);
-  REL(d_vals_b); REL(d_hist); REL(d_part_count); REL(d_part_job_off); REL(d_bitmap); REL(d_jobq); REL(d_reason);
-  REL(d_out_prio); REL(d_out_start); REL(d_out_end); REL(d_out_nalloc); REL(d_out_node); REL(d_out_ntasks);
-  REL(d_out_res); REL(d_prof); REL(d_qos); REL(d_user); REL(d_q_u32); REL(d_q_chain_off); REL(d_q_chain);
-  REL(d_q_i64); REL(d_q_valid); REL(d_part_owner); REL(d_part_list); REL(d_ntpn_max); REL(d_ntasks); REL(d_first_resv); REL(d_resv_start); REL(d_resv_end); REL(d_slot_resv);
-  REL(d_rsv_off); REL(d_rsv_id); REL(d_dead); REL(d_erase_rows); REL(d_q_off); REL(d_sched_nparts); REL(d_part_comp); REL(d_part_cidx); REL(d_sched_owner); REL(d_slot_memb); REL(d_vpart); REL(d_pd_resv); REL(d_rsv_res); REL(d_q_tres); REL(d_q_user_usage); REL(d_q_acct_usage); REL(d_q_qos_usage);
-  REL(d_st_u32); REL(d_st_rows); REL(d_st_views); REL(d_st_sched);
-#undef REL
-  for (auto& e : h->ev) cudaEventDestroy(e);
-  cudaStreamDestroy(h->stream);
-  { std::lock_guard<std::mutex> lk(g_slot_mu); g_slots_used[h->device] &= ~(1u << h->dict_slot); }
-  delete h;
-}
+void crane_sched_destroy(crane_sched_t* h) { delete h; }
 
 // Node state a running job's allocation on `node` counts against: the node's own, or —
 // for a job inside a reservation — the reservation's state of that node
@@ -489,8 +534,7 @@ static int build_layout(crane_sched* h) {
   CU(h->d_part_count.ensure(h->n_vparts + 2));
   CU(h->d_part_job_off.ensure(h->n_vparts + 2));
   CU(cudaStreamSynchronize(h->stream));
-  h->have_cluster = true;
-  h->uploaded = false;
+  h->stage = kCluster;
   h->shard_rank = 0;
   h->shard_n = 1;  // a new cluster: the partition -> rank table has to be set again
   return CRANE_OK;
@@ -508,12 +552,8 @@ int crane_sched_set_cluster(crane_sched_t* h, const crane_cluster_t* c) {
       return fail(h, CRANE_EINVAL, "cluster: gres entries must be grouped by ascending name id");
   }
   CU(cudaSetDevice(h->device));
-  h->have_cluster = false;  // state of the previous cluster / tick is void from here on
-  h->uploaded = false;
-  h->ran = false;
-  if (c->n_partitions && c->part_off[0] != 0) return fail(h, CRANE_EINVAL, "cluster: part_off[0] != 0");
-  for (uint32_t p = 0; p < c->n_partitions; ++p)
-    if (c->part_off[p + 1] < c->part_off[p]) return fail(h, CRANE_EINVAL, "cluster: part_off is not monotonic");
+  lower_stage(h, kNone);  // state of the previous cluster / tick is void from here on
+  TRY(check_offsets(h, "cluster: part_off", c->part_off, c->n_partitions));
   h->n_nodes = c->n_nodes;
   h->n_parts = c->n_partitions;
   memset(&h->dict, 0, sizeof h->dict);
@@ -538,13 +578,12 @@ int crane_sched_set_cluster(crane_sched_t* h, const crane_cluster_t* c) {
 
 int crane_sched_set_reservations(crane_sched_t* h, const crane_reservations_t* rv) {
   if (!h) return CRANE_EINVAL;
-  if (!h->have_cluster) return fail(h, CRANE_EINVAL, "set_reservations: set_cluster first");
+  TRY(require(h, kCluster, "set_reservations"));
   CU(cudaSetDevice(h->device));
   const uint32_t n = rv ? rv->n : 0;
-  if (n && (!rv->start_time || !rv->end_time || !rv->node_off)) return fail(h, CRANE_EINVAL, "reservations: null table");
-  if (n && rv->node_off[0] != 0) return fail(h, CRANE_EINVAL, "reservations: node_off[0] != 0");
+  if (n && (!rv->start_time || !rv->end_time)) return fail(h, CRANE_EINVAL, "reservations: null table");
+  if (n) TRY(check_offsets(h, "reservations: node_off", rv->node_off, n));
   for (uint32_t r = 0; r < n; ++r) {
-    if (rv->node_off[r + 1] < rv->node_off[r]) return fail(h, CRANE_EINVAL, "reservations: node_off is not monotonic");
     if (rv->end_time[r] < rv->start_time[r]) return fail(h, CRANE_EINVAL, "reservations[%u]: end before start", r);
     for (uint32_t k = rv->node_off[r]; k < rv->node_off[r + 1]; ++k) {
       if (!rv->node || !rv->res) return fail(h, CRANE_EINVAL, "reservations: null node table");
@@ -553,9 +592,7 @@ int crane_sched_set_reservations(crane_sched_t* h, const crane_reservations_t* r
         if (rv->node[k2] == rv->node[k]) return fail(h, CRANE_EINVAL, "reservations[%u]: node %u listed twice", r, rv->node[k]);
     }
   }
-  h->have_cluster = false;
-  h->uploaded = false;
-  h->ran = false;
+  lower_stage(h, kNone);
   h->n_resv = n;
   h->r_start.assign(rv ? rv->start_time : nullptr, rv ? rv->start_time + n : nullptr);
   h->r_end.assign(rv ? rv->end_time : nullptr, rv ? rv->end_time + n : nullptr);
@@ -578,7 +615,7 @@ int crane_sched_set_reservations(crane_sched_t* h, const crane_reservations_t* r
 
 int crane_sched_set_shard(crane_sched_t* h, uint32_t rank, uint32_t n_ranks, const uint32_t* part_owner) {
   if (!h) return CRANE_EINVAL;
-  if (!h->have_cluster) return fail(h, CRANE_EINVAL, "set_shard: set_cluster first");
+  TRY(require(h, kCluster, "set_shard"));
   if (n_ranks == 0 || rank >= n_ranks) return fail(h, CRANE_EINVAL, "set_shard: rank %u of %u", rank, n_ranks);
   CU(cudaSetDevice(h->device));
   h->shard_rank = rank;
@@ -608,7 +645,7 @@ int crane_sched_set_shard(crane_sched_t* h, uint32_t rank, uint32_t n_ranks, con
 
 int crane_sched_device_placements(crane_sched_t* h, crane_device_placements_t* out) {
   if (!h || !out) return CRANE_EINVAL;
-  if (!h->ran) return fail(h, CRANE_EINVAL, "device_placements: run first");
+  TRY(require(h, kRan, "device_placements"));
   out->reason = h->d_reason.p;
   out->start_time = h->d_out_start.p;
   out->end_time = h->d_out_end.p;
@@ -631,11 +668,7 @@ int h2d_at(crane_sched* h, DBuf<T>& dst, const T* src, size_t base, size_t n) {
   if (n) CU(cudaMemcpyAsync(dst.p + base, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream));
   return CRANE_OK;
 }
-#define H2D_AT(buf, src, base, n)                                  \
-  do {                                                             \
-    int rc__ = h2d_at(h, buf, src, (size_t)(base), (size_t)(n));   \
-    if (rc__ != CRANE_OK) return rc__;                             \
-  } while (0)
+#define H2D_AT(buf, src, base, n) TRY(h2d_at(h, buf, src, (size_t)(base), (size_t)(n)))
 
 // Appends the rows of `pd` to the device-resident pending table (rows keep job-id
 // order: the reference's pending map is a btree over job ids, JobScheduler.cpp:1092).
@@ -683,15 +716,8 @@ int pending_append(crane_sched* h, const crane_pending_t* pd) {
     acc += pd->node_num[i];
     if (acc > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "pending: sum(node_num) overflows");
   }
-  if ((pd->incl_off && !pd->incl_nodes && pd->incl_off[N]) || (pd->excl_off && !pd->excl_nodes && pd->excl_off[N]))
-    return fail(h, CRANE_EINVAL, "pending: node list CSR without node array");
-  for (uint32_t i = 0; i < N; ++i)
-    if ((pd->incl_off && pd->incl_off[i + 1] < pd->incl_off[i]) || (pd->excl_off && pd->excl_off[i + 1] < pd->excl_off[i]))
-      return fail(h, CRANE_EINVAL, "pending[%u]: node list offsets are not monotonic", i);
-  if (h->have_lists_incl)
-    for (uint32_t k = 0; k < pd->incl_off[N]; ++k)
-      if (pd->incl_nodes[k] >= h->n_nodes && pd->incl_nodes[k] != 0xFFFFFFFFu)  // 0xFFFFFFFF = a host the cluster does not know
-        return fail(h, CRANE_EINVAL, "pending: included node out of range");
+  if (pd->incl_off) TRY(check_node_list(h, "pending: include list", pd->incl_off, pd->incl_nodes, N));
+  if (pd->excl_off) TRY(check_node_list(h, "pending: exclude list", pd->excl_off, pd->excl_nodes, N));
   // ---- columns ----------------------------------------------------------------
   H2D_AT(h->d_partition, pd->partition, base, N);
   H2D_AT(h->d_time_limit, pd->time_limit, base, N);
@@ -748,10 +774,9 @@ int set_running(crane_sched* h, const crane_running_t* rn) {
   const uint32_t N = h->n_pending;
   const uint32_t R = rn ? rn->n : 0;
   if (R && (!rn->start_time || !rn->end_time || !rn->node_num || !rn->partition_priority || !rn->qos_priority ||
-            !rn->account || !rn->view_cpu_raw || !rn->view_mem || !rn->alloc_off))
+            !rn->account || !rn->view_cpu_raw || !rn->view_mem))
     return fail(h, CRANE_EINVAL, "running: null column");
-  for (uint32_t j = 0; j < R; ++j)
-    if (rn->alloc_off[j + 1] < rn->alloc_off[j]) return fail(h, CRANE_EINVAL, "running: alloc_off is not monotonic");
+  if (R) TRY(check_offsets(h, "running: alloc_off", rn->alloc_off, R));
   uint32_t max_account = 0;
   for (uint32_t i = 0; i < N; ++i) max_account = std::max(max_account, h->h_pd_account[i]);
   for (uint32_t k = 0; k < R; ++k) max_account = std::max(max_account, rn->account[k]);
@@ -855,20 +880,17 @@ int crane_sched_pending_reset(crane_sched_t* h) {
   h->h_alloc_off.assign(1, 0);
   h->h_pd_account.clear();
   h->h_dead.clear();
-  h->uploaded = false;
-  h->ran = false;
+  lower_stage(h, kCluster);
   return CRANE_OK;
 }
 
 int crane_sched_pending_append(crane_sched_t* h, const crane_pending_t* rows, uint32_t* first_row) {
   if (!h || !rows) return CRANE_EINVAL;
-  if (!h->have_cluster) return fail(h, CRANE_EINVAL, "pending_append: set_cluster first");
+  TRY(require(h, kCluster, "pending_append"));
   CU(cudaSetDevice(h->device));
-  h->uploaded = false;  // the running table and the work buffers follow with crane_sched_set_running
-  h->ran = false;
+  lower_stage(h, kCluster);  // the running table and the work buffers follow with crane_sched_set_running
   const uint32_t base = h->n_pending;
-  int rc = pending_append(h, rows);
-  if (rc != CRANE_OK) return rc;
+  TRY(pending_append(h, rows));
   if (first_row) *first_row = base;
   return CRANE_OK;
 }
@@ -878,8 +900,7 @@ int crane_sched_pending_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n
   CU(cudaSetDevice(h->device));
   for (uint32_t k = 0; k < n; ++k)
     if (rows[k] >= h->n_pending) return fail(h, CRANE_EINVAL, "pending_erase: row %u out of range", rows[k]);
-  h->uploaded = false;
-  h->ran = false;
+  lower_stage(h, kCluster);
   if (!n) return CRANE_OK;
   for (uint32_t k = 0; k < n; ++k)
     if (!h->h_dead[rows[k]]) { h->h_dead[rows[k]] = 1; h->n_dead++; }
@@ -892,39 +913,35 @@ int crane_sched_pending_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n
 
 int crane_sched_set_running(crane_sched_t* h, const crane_running_t* rn) {
   if (!h) return CRANE_EINVAL;
-  if (!h->have_cluster) return fail(h, CRANE_EINVAL, "set_running: set_cluster first");
+  TRY(require(h, kCluster, "set_running"));
   CU(cudaSetDevice(h->device));
-  h->uploaded = false;
-  h->ran = false;
-  int rc = set_running(h, rn);
-  if (rc != CRANE_OK) return rc;
-  h->uploaded = true;
+  lower_stage(h, kCluster);
+  TRY(set_running(h, rn));
+  h->stage = kUploaded;
   return CRANE_OK;
 }
 
 int crane_sched_upload(crane_sched_t* h, const crane_running_t* rn, const crane_pending_t* pd) {
   if (!h || !pd) return CRANE_EINVAL;
-  if (!h->have_cluster) return fail(h, CRANE_EINVAL, "upload: set_cluster first");
+  TRY(require(h, kCluster, "upload"));
   CU(cudaSetDevice(h->device));
-  h->uploaded = false;  // a failed upload leaves nothing runnable behind
-  h->ran = false;
-  CU(cudaEventRecord(h->ev[0], h->stream));
+  lower_stage(h, kCluster);  // a failed upload leaves nothing runnable behind
+  CU(cudaEventRecord(h->ev[kEvH2dBegin], h->stream));
   crane_sched_pending_reset(h);
   int rc = pending_append(h, pd);
   if (rc != CRANE_OK) { crane_sched_pending_reset(h); return rc; }
-  rc = set_running(h, rn);
-  if (rc != CRANE_OK) return rc;
-  CU(cudaEventRecord(h->ev[1], h->stream));
+  TRY(set_running(h, rn));
+  CU(cudaEventRecord(h->ev[kEvH2dEnd], h->stream));
   h->h2d_timed = true;
-  h->uploaded = true;
-  h->ran = false;
+  h->stage = kUploaded;
   return CRANE_OK;
 }
 
 int crane_sched_run(crane_sched_t* h, int64_t now) {
   if (!h) return CRANE_EINVAL;
-  if (!h->uploaded) return fail(h, CRANE_EINVAL, "run: upload first");
+  TRY(require(h, kUploaded, "run"));
   CU(cudaSetDevice(h->device));
+  lower_stage(h, kUploaded);  // the previous run's outputs are void from here on
   (void)cudaGetLastError();  // a stale error of an earlier, unrelated call in this process is not this run's
   cudaStream_t st = h->stream;
   const uint32_t N = h->n_pending, R = h->n_running;
@@ -1016,7 +1033,7 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
   out.alloc_res = h->d_out_res.p;
 
   // ---- node state / timelines (R2,R3,R4) -----------------------------------
-  CU(cudaEventRecord(h->ev[2], st));
+  CU(cudaEventRecord(h->ev[kEvRunBegin], st));
   if (h->total_alloc) {  // allocation slots of jobs without a placement read as zero
     CU(cudaMemsetAsync(h->d_out_node.p, 0, sizeof(uint32_t) * h->total_alloc, st));
     CU(cudaMemsetAsync(h->d_out_ntasks.p, 0, sizeof(uint32_t) * h->total_alloc, st));
@@ -1026,7 +1043,7 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     CRANE_LAUNCH(k_node_init, (h->n_slots + 127) / 128, 128, 0, st, cl, rn, tl, now, h->cfg.max_jobs_per_node, h->cfg.cost_policy);
     h->timing.kernel_launches++;
   }
-  CU(cudaEventRecord(h->ev[3], st));
+  CU(cudaEventRecord(h->ev[kEvInitEnd], st));
 
   // ---- priority + queue (R5,R6) --------------------------------------------
   uint32_t nq_cap = std::min<uint32_t>(N, h->cfg.scheduled_batch_size);
@@ -1058,10 +1075,8 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     CRANE_LAUNCH(k_priority, (N + 255) / 256, 256, 0, st, pd, pc, now, h->d_bounds.p, h->d_acc_service.p,
                  h->d_prio.p, h->d_keys_a.p, h->d_vals_a.p);
     h->timing.kernel_launches++;
-    if (pc.type != 0 || h->n_dead) {  // (FIFO keeps input order; erased rows only have to go behind the live ones)
-      int rc = radix_sort(h, N, pc.type != 0 ? 64 : 8, &keys, &vals);
-      if (rc != CRANE_OK) return rc;
-    }
+    if (pc.type != 0 || h->n_dead)  // (FIFO keeps input order; erased rows only have to go behind the live ones)
+      TRY(radix_sort(h, N, pc.type != 0 ? 64 : 8, &keys, &vals));
     // keys2 go to the buffer not holding `vals`
     uint64_t* key2 = h->d_keys_a.p;
     uint32_t* order = vals;
@@ -1078,8 +1093,7 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     while ((1ull << bits) < (uint64_t)h->n_vparts + 2) bits += 8;
     uint64_t* k2s;
     uint32_t* queue;
-    int rc = radix_sort(h, N, bits, &k2s, &queue);
-    if (rc != CRANE_OK) return rc;
+    TRY(radix_sort(h, N, bits, &k2s, &queue));
     h->d_queue = queue;
     if (nq_cap) {
       // n_queued <= nq_cap lives on the device (part_job_off[n_parts]); the
@@ -1091,7 +1105,7 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     CRANE_LAUNCH(k_part_offsets, 1, 32, 0, st, h->d_part_count.p, h->n_vparts, h->d_part_job_off.p);
     h->timing.kernel_launches++;
   }
-  CU(cudaEventRecord(h->ev[4], st));
+  CU(cudaEventRecord(h->ev[kEvPrioEnd], st));
 
   // ---- capability bitmap (R7 predicate + R8) -------------------------------
   if (nq_cap && h->n_vparts) {
@@ -1101,7 +1115,7 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
                  h->shard_n > 1 ? h->d_sched_owner.p : nullptr, h->shard_rank, (uint32_t)h->dict_slot);
     h->timing.kernel_launches++;
   }
-  CU(cudaEventRecord(h->ev[5], st));
+  CU(cudaEventRecord(h->ev[kEvFeasEnd], st));
 
   // ---- sequential commit (R7,R9,R10,R11) -----------------------------------
   if (nq_cap && h->n_vparts) {
@@ -1130,15 +1144,15 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
       h->timing.kernel_launches++;
     }
   }
-  CU(cudaEventRecord(h->ev[6], st));
+  CU(cudaEventRecord(h->ev[kEvRunEnd], st));
   CU(cudaGetLastError());
-  h->ran = true;
+  h->stage = kRan;
   return CRANE_OK;
 }
 
 int crane_sched_fetch(crane_sched_t* h, crane_placements_t* out) {
   if (!h || !out) return CRANE_EINVAL;
-  if (!h->ran) return fail(h, CRANE_EINVAL, "fetch: run first");
+  TRY(require(h, kRan, "fetch"));
   CU(cudaSetDevice(h->device));
   cudaStream_t st = h->stream;
   const uint32_t N = h->n_pending;
@@ -1160,27 +1174,20 @@ int crane_sched_fetch(crane_sched_t* h, crane_placements_t* out) {
     CU(cudaMemcpyAsync(out->alloc_res, h->d_out_res.p, sizeof(Row) * h->total_alloc, cudaMemcpyDeviceToHost, st));
   }
   memcpy(out->alloc_off, h->h_alloc_off.data(), sizeof(uint32_t) * ((size_t)N + 1));
-  CU(cudaEventRecord(h->ev[7], st));
+  CU(cudaEventRecord(h->ev[kEvD2hEnd], st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  float ms = 0;
   // (the upload events exist only after crane_sched_upload: a resident table is filled piecewise)
-  if (h->h2d_timed) { cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]); h->timing.h2d_ms = ms; } else h->timing.h2d_ms = 0.f;
-  cudaEventElapsedTime(&ms, h->ev[2], h->ev[3]); h->timing.init_ms = ms;
-  cudaEventElapsedTime(&ms, h->ev[3], h->ev[4]); h->timing.priority_ms = ms;
-  cudaEventElapsedTime(&ms, h->ev[4], h->ev[5]); h->timing.feas_ms = ms;
-  cudaEventElapsedTime(&ms, h->ev[5], h->ev[6]); h->timing.commit_ms = ms;
-  cudaEventElapsedTime(&ms, h->ev[6], h->ev[7]); h->timing.d2h_ms = ms;
-  cudaEventElapsedTime(&ms, h->ev[2], h->ev[6]); h->timing.total_ms = ms;
+  h->timing.h2d_ms = h->h2d_timed ? elapsed_ms(h, kEvH2dBegin, kEvH2dEnd) : 0.f;
+  read_run_times(h);
+  h->timing.d2h_ms = elapsed_ms(h, kEvRunEnd, kEvD2hEnd);
   return CRANE_OK;
 }
 
 int crane_sched_node_select(crane_sched_t* h, int64_t now, const crane_running_t* running,
                             const crane_pending_t* pending, crane_placements_t* out) {
-  int rc = crane_sched_upload(h, running, pending);
-  if (rc != CRANE_OK) return rc;
-  rc = crane_sched_run(h, now);
-  if (rc != CRANE_OK) return rc;
+  TRY(crane_sched_upload(h, running, pending));
+  TRY(crane_sched_run(h, now));
   return crane_sched_fetch(h, out);
 }
 
@@ -1189,22 +1196,14 @@ int crane_sched_sync(crane_sched_t* h, float* run_ms) {
   CU(cudaSetDevice(h->device));
   CU(cudaStreamSynchronize(h->stream));
   CU(cudaGetLastError());
-  if (h->ran) {
-    float ms = 0;
-    cudaEventElapsedTime(&ms, h->ev[2], h->ev[3]); h->timing.init_ms = ms;
-    cudaEventElapsedTime(&ms, h->ev[3], h->ev[4]); h->timing.priority_ms = ms;
-    cudaEventElapsedTime(&ms, h->ev[4], h->ev[5]); h->timing.feas_ms = ms;
-    cudaEventElapsedTime(&ms, h->ev[5], h->ev[6]); h->timing.commit_ms = ms;
-    cudaEventElapsedTime(&ms, h->ev[2], h->ev[6]); h->timing.total_ms = ms;
-    if (run_ms) *run_ms = ms;
-  } else if (run_ms) {
-    *run_ms = 0.f;
-  }
+  if (h->stage == kRan) read_run_times(h);
+  if (run_ms) *run_ms = h->stage == kRan ? h->timing.total_ms : 0.f;
   return CRANE_OK;
 }
 
 int crane_sched_debug_profile(crane_sched_t* h, unsigned long long* dst, size_t cap) {
-  if (!h || !h->ran || !dst) return CRANE_EINVAL;
+  if (!h || !dst) return CRANE_EINVAL;
+  TRY(require(h, kRan, "debug_profile"));
   CU(cudaSetDevice(h->device));
   size_t n = std::min(cap, (size_t)h->n_vparts * 16);
   CU(cudaStreamSynchronize(h->stream));
@@ -1214,7 +1213,7 @@ int crane_sched_debug_profile(crane_sched_t* h, unsigned long long* dst, size_t 
 
 int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_t* reason) {
   if (!h || !qt || !reason) return CRANE_EINVAL;
-  if (!h->ran) return fail(h, CRANE_EINVAL, "qos_filter: run first");
+  TRY(require(h, kRan, "qos_filter"));
   if (!h->have_qos_cols) return fail(h, CRANE_EINVAL, "qos_filter: pending.qos / pending.user were not uploaded");
   CU(cudaSetDevice(h->device));
   const uint32_t N = h->n_pending, Q = qt->n_qos, U = qt->n_users, A = qt->n_accounts;
@@ -1222,13 +1221,14 @@ int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_
   if (A > 65535) return fail(h, CRANE_ENOSYS, "qos_filter: more than 65535 accounts");
   if (!qt->valid || !qt->max_jobs_per_user || !qt->max_jobs_per_account || !qt->max_jobs ||
       !qt->max_cpus_per_user_raw || !qt->max_wall || !qt->max_tres_per_user || !qt->max_tres_per_account ||
-      !qt->max_tres || !qt->chain_off || !qt->user_usage || !qt->qos_usage || (A && !qt->account_usage))
+      !qt->max_tres || !qt->user_usage || !qt->qos_usage || (A && !qt->account_usage))
     return fail(h, CRANE_EINVAL, "qos_filter: null column");
+  TRY(check_offsets(h, "qos_filter: chain_off", qt->chain_off, N));
   // the levels of one job are checked lane-parallel: user + chain + qos <= 32
   // lanes, and one usage entry per lane (a chain never repeats an account)
   for (uint32_t i = 0; i < N; ++i) {
     const uint32_t c0 = qt->chain_off[i], c1 = qt->chain_off[i + 1];
-    if (c1 < c0 || c1 - c0 > 30) return fail(h, CRANE_ENOSYS, "qos_filter: pending[%u]: account chain longer than 30", i);
+    if (c1 - c0 > 30) return fail(h, CRANE_ENOSYS, "qos_filter: pending[%u]: account chain longer than 30", i);
     for (uint32_t a = c0; a < c1; ++a) {
       if (qt->chain_acct[a] >= A) return fail(h, CRANE_EINVAL, "qos_filter: pending[%u]: account out of range", i);
       for (uint32_t b = c0; b < a; ++b)
@@ -1277,13 +1277,12 @@ int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_
     // the jobs the pass walks, grouped by qos in job-id order: key + stable radix sort
     const int bits = Q < 255 ? 8 : 16;
     const uint64_t sentinel = (1ull << bits) - 1;
-    CU(cudaEventRecord(h->ev[8], h->stream));
+    CU(cudaEventRecord(h->ev[kEvQosBegin], h->stream));
     CU(h->d_keys_a.ensure(N)); CU(h->d_keys_b.ensure(N)); CU(h->d_vals_a.ensure(N)); CU(h->d_vals_b.ensure(N));
     CRANE_LAUNCH(k_qos_keys, (N + 255) / 256, 256, 0, h->stream, q, h->d_keys_a.p, h->d_vals_a.p, sentinel);
     uint64_t* keys;
     uint32_t* list;
-    int rc = radix_sort(h, N, bits, &keys, &list);
-    if (rc != CRANE_OK) return rc;
+    TRY(radix_sort(h, N, bits, &keys, &list));
     CU(h->d_q_off.ensure((size_t)Q + 1));
     CRANE_LAUNCH(k_qos_offsets, (Q + 1 + 127) / 128, 128, 0, h->stream, keys, N, Q, h->d_q_off.p);
     // the usage column of one qos in shared memory when it fits beside the job buffers
@@ -1294,7 +1293,7 @@ int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_
     CU(cudaFuncSetAttribute(k_qos_chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
     CRANE_LAUNCH(k_qos_chain, Q, kQosThreads, dyn, h->stream, q, h->dict, list, h->d_q_off.p, in_smem);
     CU(cudaGetLastError());
-    CU(cudaEventRecord(h->ev[9], h->stream));
+    CU(cudaEventRecord(h->ev[kEvQosEnd], h->stream));
     h->timing.kernel_launches += 3;
   }
   if (N) CU(cudaMemcpyAsync(reason, h->d_reason.p, N, cudaMemcpyDeviceToHost, h->stream));
@@ -1302,22 +1301,17 @@ int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_
   if ((size_t)A * Q) CU(cudaMemcpyAsync(qt->account_usage, h->d_q_acct_usage.p, (size_t)A * Q * sizeof(crane_meta_resource_t), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaMemcpyAsync(qt->qos_usage, h->d_q_qos_usage.p, (size_t)Q * sizeof(crane_meta_resource_t), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
-  h->timing.qos_ms = 0.f;
-  if (N) cudaEventElapsedTime(&h->timing.qos_ms, h->ev[8], h->ev[9]);
+  h->timing.qos_ms = N ? elapsed_ms(h, kEvQosBegin, kEvQosEnd) : 0.f;
   return CRANE_OK;
 }
 
 int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, const crane_steps_t* st,
                                crane_step_placements_t* out, float* device_ms) {
   if (!h || !jb || !st || !out) return CRANE_EINVAL;
-  if (!h->have_cluster) return fail(h, CRANE_EINVAL, "schedule_steps: set_cluster first");
+  TRY(require(h, kCluster, "schedule_steps"));
   const uint32_t J = jb->n_jobs;
-  if (!jb->node_off || !jb->step_off) return fail(h, CRANE_EINVAL, "step jobs: null offsets");
-  if (jb->node_off[0] != 0 || jb->step_off[0] != 0) return fail(h, CRANE_EINVAL, "step jobs: offsets must start at 0");
-  for (uint32_t j = 0; j < J; ++j) {
-    if (jb->node_off[j + 1] < jb->node_off[j] || jb->step_off[j + 1] < jb->step_off[j])
-      return fail(h, CRANE_EINVAL, "step jobs: offsets are not monotonic");
-  }
+  TRY(check_offsets(h, "step jobs: node_off", jb->node_off, J));
+  TRY(check_offsets(h, "step jobs: step_off", jb->step_off, J));
   const uint32_t E = jb->node_off[J], S = jb->step_off[J];
   if (st->n != S) return fail(h, CRANE_EINVAL, "steps: n (%u) != step_off[n_jobs] (%u)", st->n, S);
   if (E && (!jb->node || !jb->avail)) return fail(h, CRANE_EINVAL, "step jobs: null node table");
@@ -1344,17 +1338,8 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
     trows += nt;
   }
   if (nrows > 0xfffffff0ull || trows > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "steps: too many node / task rows");
-  for (int l = 0; l < 2; ++l) {
-    const uint32_t* off = l ? st->excl_off : st->incl_off;
-    const uint32_t* nodes = l ? st->excl_nodes : st->incl_nodes;
-    if (!off) continue;
-    if (off[0] != 0) return fail(h, CRANE_EINVAL, "steps: node list offsets must start at 0");
-    for (uint32_t s = 0; s < S; ++s)
-      if (off[s + 1] < off[s]) return fail(h, CRANE_EINVAL, "steps[%u]: node list offsets are not monotonic", s);
-    if (off[S] && !nodes) return fail(h, CRANE_EINVAL, "steps: node list CSR without node array");
-    for (uint32_t k = 0; k < off[S]; ++k)
-      if (nodes[k] >= h->n_nodes && nodes[k] != 0xFFFFFFFFu) return fail(h, CRANE_EINVAL, "steps: listed node out of range");
-  }
+  if (st->incl_off) TRY(check_node_list(h, "steps: include list", st->incl_off, st->incl_nodes, S));
+  if (st->excl_off) TRY(check_node_list(h, "steps: exclude list", st->excl_off, st->excl_nodes, S));
   if ((J && !out->placed) || (S && (!out->scheduled || !out->node_off || !out->task_off)) || !out->node_off || !out->task_off ||
       (nrows && (!out->alloc_node || !out->alloc_ntasks || !out->alloc_res)) || (trows && (!out->task_node || !out->task_res)))
     return fail(h, CRANE_EINVAL, "step placements: null column");
@@ -1405,13 +1390,13 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
               st->incl_off ? du + o_io : nullptr, du + o_in, st->excl_off ? du + o_eo : nullptr, du + o_en};
   StepOutDev dout{du + o_placed, h->d_st_sched.p, du + o_ooff, du + o_anode, du + o_antasks, dr + E,
                   du + o_toff, du + o_tnode, dr + E + nrows};
-  CU(cudaEventRecord(h->ev[10], sm));
+  CU(cudaEventRecord(h->ev[kEvStepsBegin], sm));
   if (J) {
     const uint32_t grid = std::min<uint32_t>((J + kStepWarps - 1) / kStepWarps, 16 * h->n_sm);
     CRANE_LAUNCH(k_steps, grid, 32 * kStepWarps, 0, sm, dj, ds, dout, (uint32_t)h->dict_slot);
     CU(cudaGetLastError());
   }
-  CU(cudaEventRecord(h->ev[11], sm));
+  CU(cudaEventRecord(h->ev[kEvStepsEnd], sm));
   if (J) CU(cudaMemcpyAsync(out->placed, du + o_placed, J * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
   if (S) CU(cudaMemcpyAsync(out->scheduled, h->d_st_sched.p, S, cudaMemcpyDeviceToHost, sm));
   if (nrows) {
@@ -1426,11 +1411,7 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
   if (E) CU(cudaMemcpyAsync(jb->avail, dr, E * sizeof(Row), cudaMemcpyDeviceToHost, sm));
   CU(cudaStreamSynchronize(sm));
   CU(cudaGetLastError());
-  if (device_ms) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, h->ev[10], h->ev[11]);
-    *device_ms = ms;
-  }
+  if (device_ms) *device_ms = elapsed_ms(h, kEvStepsBegin, kEvStepsEnd);
   return CRANE_OK;
 }
 
@@ -1442,7 +1423,8 @@ int crane_sched_get_timing(const crane_sched_t* h, crane_sched_timing_t* t) {
 
 int crane_sched_debug_bitmap(crane_sched_t* h, uint32_t* dst, size_t cap_words, uint32_t* rows,
                              uint32_t* words_per_row) {
-  if (!h || !h->ran) return CRANE_EINVAL;
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kRan, "debug_bitmap"));
   CU(cudaSetDevice(h->device));
   uint32_t nq = 0;
   CU(cudaMemcpy(&nq, h->d_part_job_off.p + h->n_vparts, sizeof(uint32_t), cudaMemcpyDeviceToHost));

@@ -24,6 +24,8 @@
  *     PublicHeader.h:412-479,540-558) are bit masks: core bit i = core id i;
  *     slot bit i of gres entry e = the i-th slot (lexicographic slot-path
  *     order) of that (name,type) on that node.
+ *   - every `*_off` input array is a CSR offsets array of n+1 entries that
+ *     starts at 0 and never decreases; anything else is CRANE_EINVAL.
  *   - all functions return 0 on success or a negative CRANE_E* code; they
  *     never throw and never fall back to a CPU implementation.
  */
