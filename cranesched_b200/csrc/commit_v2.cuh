@@ -21,7 +21,7 @@
 //             in its scratch word, the next job's list is prefetched). A job
 //             that could use a node taken by an earlier job of the batch at
 //             that node's NEW place in the order ends the batch: it needs the
-//             updated timeline. Warps 1-7 meanwhile test every slot's first
+//             updated timeline (a node the earlier job filled is no candidate). Warps 1-7 meanwhile test every slot's first
 //             guess (the entry taken if the jobs before take the entries before);
 //   evaluate  group w runs the exact test of task w = (job, node) without
 //             touching state: window minimum (JobScheduler.cpp:5285-5334) or
@@ -490,11 +490,15 @@ __device__ __forceinline__ void jsel_load(const JobQ& jq, const uint32_t* bits, 
 __device__ __forceinline__ bool capable2(const Smem2& sm, const JSel2& js, uint32_t q) {
   return ((js.bits[q >> 5] >> (q & 31)) & 1u) && !sm.skip[q];
 }
-// necessary condition of the window test, on the first segment's counts
-__device__ __forceinline__ bool prefilter2(const Smem2& sm, const JSel2& js, uint32_t q) {
+// necessary condition of the window test, on the first segment's counts (cpu0: its
+// cpu, which a job of the batch that starts now on the node lowers)
+__device__ __forceinline__ bool prefilter_cpu2(const Smem2& sm, const JSel2& js, uint32_t q, int64_t cpu0) {
   if (js.exclusive) return true;
-  if (sm.cpu0[q] < js.req_cpu) return false;
+  if (cpu0 < js.req_cpu) return false;
   return !js.has_gres || (sm.gcnt && gres_counts_ok(sm.gcnt[q], js.spec8, js.gnames, js.name_need, C_DICT2));
+}
+__device__ __forceinline__ bool prefilter2(const Smem2& sm, const JSel2& js, uint32_t q) {
+  return prefilter_cpu2(sm, js, q, sm.cpu0[q]);
 }
 __device__ __forceinline__ bool bounds_admit2(const JSel2& js, long long mcpu, long long mcpug, unsigned long long mg) {
   if (js.exclusive) return true;
@@ -1603,8 +1607,12 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
           // ends before a job whose candidates were taken by the jobs before it, or
           // for which a taken node, at its NEW key, sorts before the job's last pick
           // while it still is a candidate: that node would be among the first K of
-          // the updated order, so the job has to see the node's update first.
+          // the updated order, so the job has to see the node's update first. "Still a
+          // candidate" is judged on the node's first segment after the earlier job: the
+          // timeline starts at `now`, so a job that starts now takes its cpu out of that
+          // segment, and a node it filled is no clash.
           uint32_t tv = 0xffffu, tslot = 0xffffffffu;  // my task slot: node (0xffff = void), job
+          int64_t tcpu = 0;                            // cpu of my node's first segment after my slot's job
           double tnc = 0.0;
           uint32_t njr_l = nj;
           uint32_t nw = s2_jw[0];
@@ -1638,7 +1646,7 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
               JSel2 jt;
               const uint32_t slot = s2_bj[t].slot;
               jsel_load(s2_jobs[slot], sm.bits_ring + (size_t)slot * words, jt);
-              const bool rel = ((cl >> lane) & 1u) && capable2(sm, jt, tv) && (mode || prefilter2(sm, jt, tv));
+              const bool rel = ((cl >> lane) & 1u) && capable2(sm, jt, tv) && (mode || prefilter_cpu2(sm, jt, tv, tcpu));
               cl = __ballot_sync(kFullMask, rel);
             }
             if (cl) {
@@ -1656,7 +1664,14 @@ __global__ void __launch_bounds__(kT2, 1) k_commit2(Commit2Args a) {
             const uint32_t src = mine ? (K == 1 ? kth : nth_set_bit(cm, lane - tf + 1u)) : 0u;
             const uint32_t pq = __shfl_sync(kFullMask, lq, (int)(src & 31u));
             const double pnc = __shfl_sync(kFullMask, nc, (int)(src & 31u));
-            if (mine) { tv = pq; tnc = pnc; }
+            if (mine) {
+              tv = pq; tnc = pnc;
+              tcpu = sm.cpu0[pq];
+              if (!mode) {  // starts now (exclusive: takes res_total)
+                const JobQ& jq = s2_jobs[s2_bj[t].slot];
+                tcpu -= jq_exclusive(jq) ? node_total_cpu2(pq) : jq.req.cpu_raw;
+              }
+            }
             __syncwarp();
           }
           const uint32_t NTl = njr_l ? ((s2_jw[njr_l - 1] >> 8) & 0xffu) + (s2_jw[njr_l - 1] & 0xffu) : 0u;

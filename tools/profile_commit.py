@@ -25,9 +25,13 @@ t = s.timing()
 prof = s.debug_profile()
 jobs = np.bincount(pd.partition[pd.partition < cl.n_partitions], minlength=cl.n_partitions)
 print(json.dumps({k: round(v, 3) for k, v in t.items()}))
+crit = max(range(cl.n_partitions), key=lambda p: sum(int(prof[p, i]) for i in TIMED))
 for p in range(cl.n_partitions):
     tot = sum(int(prof[p, i]) for i in TIMED)
-    print("partition %d: %d jobs, %.0f cycles/job, total %.1f Mcycles" % (p, jobs[p], tot / max(jobs[p], 1), tot / 1e6))
+    nb, nbj = int(prof[p, 14]), int(prof[p, 13])
+    print("partition %d: %d jobs, %.0f cycles/job, total %.1f Mcycles%s" % (p, jobs[p], tot / max(jobs[p], 1), tot / 1e6,
+                                                                          "  <- critical CTA" if p == crit else ""))
+    print("   %-20s %10d batches, %.2f jobs per batch" % ("batches", nb, nbj / max(nb, 1)))
     for i, n in enumerate(NAMES):
         v = int(prof[p, i])
         if i in TIMED:
@@ -37,5 +41,5 @@ for p in range(cl.n_partitions):
                 print("   %-20s %10.2f per job" % (n, (v & 0xffffffff) / max(jobs[p], 1)))
                 print("   %-20s %10.2f per job" % ("#jobs on the one-job path", (v >> 32) / max(jobs[p], 1)))
             else:
-                print("   %-20s %10.2f per job" % (n, v / max(jobs[p], 1)))
+                print("   %-20s %10d  (%.2f per job)" % (n, v, v / max(jobs[p], 1)))
 s.close()
