@@ -28,6 +28,8 @@ REASON_PRIORITY = 1
 REASON_RESOURCE = 2
 REASON_RESERVED = 3
 REASON_PART_NOT_FOUND = 4
+REASON_RESV_NOT_FOUND = 5
+REASON_ERASED = 255  # a row removed from the device-resident pending table
 REASON_QOS_CPU = 16
 REASON_QOS_JOBS = 17
 REASON_QOS_WALL = 18
@@ -339,6 +341,53 @@ class Running:
     @property
     def n(self):
         return len(self.start_time)
+
+    def take(self, idx) -> "Running":
+        """Rows `idx` (in the given order) as a table of their own."""
+        idx = np.asarray(idx, np.int64)
+        nn = (self.alloc_off[1:] - self.alloc_off[:-1]).astype(np.int64)[idx]
+        off = np.zeros(len(idx) + 1, np.uint32)
+        off[1:] = np.cumsum(nn)
+        ent = np.repeat(self.alloc_off[:-1][idx].astype(np.int64) - off[:-1], nn) + np.arange(int(off[-1]))
+        return Running(self.start_time[idx], self.end_time[idx], self.node_num[idx], self.partition_priority[idx],
+                       self.qos_priority[idx], self.account[idx], self.view_cpu_raw[idx], self.view_mem[idx], off,
+                       self.alloc_node[ent], self.alloc_res[ent],
+                       None if self.reservation is None else self.reservation[idx])
+
+    @staticmethod
+    def concat(a: "Running", b: "Running") -> "Running":
+        """The rows of `a`, then the rows of `b`."""
+        cols = {f: np.concatenate([getattr(a, f), getattr(b, f)])
+                for f in a.__dataclass_fields__ if f not in ("alloc_off", "reservation")}
+        cols["alloc_off"] = np.concatenate([a.alloc_off, a.alloc_off[-1] + b.alloc_off[1:]])
+        if a.reservation is not None or b.reservation is not None:
+            none = lambda t: np.full(t.n, 0xFFFFFFFF, np.uint32)
+            cols["reservation"] = np.concatenate([none(a) if a.reservation is None else a.reservation,
+                                                  none(b) if b.reservation is None else b.reservation])
+        return Running(**cols)
+
+    @staticmethod
+    def started(pending: "Pending", placements: "Placements", rows) -> "Running":
+        """The running jobs that pending rows `rows` (in this order) become when a run
+        with `placements` starts them (JobScheduler.cpp:1273-1305): start / end time from
+        the placement, node_num, partition_priority, qos_priority, account and
+        reservation from the pending row, the placement rows as the allocation and
+        their sum as the view (allocated_res_view += AllocatedRes())."""
+        rows = np.asarray(rows, np.int64)
+        nn = pending.node_num[rows].astype(np.int64)
+        off = np.zeros(len(rows) + 1, np.uint32)
+        off[1:] = np.cumsum(nn)
+        ent = np.repeat(placements.alloc_off[rows].astype(np.int64) - off[:-1], nn) + np.arange(int(off[-1]))
+        res = placements.alloc_res[ent]
+        job = np.repeat(np.arange(len(rows)), nn)
+        cpu = np.zeros(len(rows), np.int64)
+        mem = np.zeros(len(rows), np.uint64)
+        np.add.at(cpu, job, res["cpu_raw"])
+        np.add.at(mem, job, res["mem"])
+        return Running(placements.start_time[rows], placements.end_time[rows], pending.node_num[rows],
+                       pending.partition_priority[rows], pending.qos_priority[rows], pending.account[rows],
+                       cpu, mem, off, placements.alloc_node[ent], res,
+                       None if pending.reservation is None else pending.reservation[rows])
 
     def as_c(self) -> RunningC:
         return RunningC(

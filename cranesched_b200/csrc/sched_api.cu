@@ -30,6 +30,7 @@
 #include "commit_v2.cuh"
 #include "qos_kernels.cuh"
 #include "step_kernels.cuh"
+#include "running_kernels.cuh"
 
 using namespace crane;
 
@@ -85,6 +86,7 @@ enum Ev {
   kEvRunBegin, kEvInitEnd, kEvPrioEnd, kEvFeasEnd, kEvRunEnd, kEvD2hEnd,  // run, fetch
   kEvQosBegin, kEvQosEnd,                                                  // qos_filter
   kEvStepsBegin, kEvStepsEnd,                                              // schedule_steps
+  kEvKeepBegin, kEvKeepEnd,                                                // keep_running
   kNumEv
 };
 
@@ -158,10 +160,23 @@ struct crane_sched {
   DBuf<double> d_mandated;
   DBuf<View> d_req_node, d_req_task, d_req_total;
   DBuf<uint32_t> d_incl_off, d_incl_nodes, d_excl_off, d_excl_nodes;
-  // running (device)
+  // device-resident running table: rows keep their index until the table is replaced,
+  // an erased row is a tombstone; host mirrors of the small columns
+  uint32_t n_rr = 0, n_rr_dead = 0;
+  std::vector<uint32_t> h_rr_alloc_off = {0}, h_rr_account;
+  std::vector<uint8_t> h_rr_dead;
+  uint32_t rr_node_bound = 0;  // every node index of a row is below this
+  bool rr_dirty = true;        // rows or the node-state layout changed since the last regroup
+  DBuf<int64_t> d_rr_start, d_rr_end, d_rr_cpu;
+  DBuf<uint32_t> d_rr_node_num, d_rr_part_prio, d_rr_qos_prio, d_rr_account, d_rr_resv, d_rr_alloc_off, d_rr_alloc_node;
+  DBuf<uint64_t> d_rr_mem;
+  DBuf<Row> d_rr_alloc_res;
+  DBuf<uint8_t> d_rr_dead;
+  DBuf<uint32_t> d_r_node_off, d_r_node, d_flag, d_start_rows;
+  // the tick's view of the live rows (RunningDev), built by the regroup
   DBuf<int64_t> d_rn_start, d_rn_end, d_rn_cpu, d_rn_slot_end;
   DBuf<uint32_t> d_rn_node_num, d_rn_part_prio, d_rn_qos_prio, d_rn_account, d_rn_slot_off, d_rn_acc_off, d_rn_acc_job;
-  DBuf<uint64_t> d_rn_mem;
+  DBuf<uint64_t> d_rn_mem, d_rn_acc_key;
   DBuf<Row> d_rn_slot_res;
   DBuf<uint8_t> d_acc_present;
   // work buffers
@@ -362,19 +377,6 @@ int crane_sched_create(const crane_sched_config_t* cfg, int device, crane_sched_
 
 void crane_sched_destroy(crane_sched_t* h) { delete h; }
 
-// Node state a running job's allocation on `node` counts against: the node's own, or —
-// for a job inside a reservation — the reservation's state of that node
-// (JobScheduler.cpp:5715-5741)
-static uint32_t running_slot(const crane_sched* h, const crane_running_t* rn, uint32_t j, uint32_t node) {
-  const uint32_t rv = rn->reservation ? rn->reservation[j] : 0xffffffffu;
-  if (rv == 0xffffffffu) return h->h_node_slot[node];
-  if (rv >= h->n_resv) return 0xffffffffu;  // the reference logs an error and skips the job
-  const uint32_t lo = h->r_node_off[rv], hi = h->r_node_off[rv + 1];
-  const auto it = std::lower_bound(h->r_node.begin() + lo, h->r_node.begin() + hi, node);
-  if (it == h->r_node.begin() + hi || *it != node) return 0xffffffffu;
-  return h->h_part_base[h->n_comp + rv] + (uint32_t)(it - (h->r_node.begin() + lo));
-}
-
 // Slot layout of the node states: the usable nodes of every partition (contiguous per
 // partition), then the nodes of every reservation; device copies of the cluster tables.
 static int build_layout(crane_sched* h) {
@@ -523,6 +525,8 @@ static int build_layout(crane_sched* h) {
   H2D(h->d_rsv_res, rsv_res.data(), rsv_res.size());
   H2D(h->d_resv_start, h->r_start.data(), h->r_start.size());
   H2D(h->d_resv_end, h->r_end.data(), h->r_end.size());
+  H2D(h->d_r_node_off, h->r_node_off.data(), h->r_node_off.size());
+  H2D(h->d_r_node, h->r_node.data(), h->r_node.size());
   CU(cudaMemcpyToSymbolAsync(c_dicts, &h->dict, sizeof(GresDict), (size_t)h->dict_slot * sizeof(GresDict), cudaMemcpyHostToDevice, h->stream));
   size_t ns = std::max<uint32_t>(h->n_slots, 1);
   CU(h->d_tl_n.ensure(ns));
@@ -535,6 +539,7 @@ static int build_layout(crane_sched* h) {
   CU(h->d_part_job_off.ensure(h->n_vparts + 2));
   CU(cudaStreamSynchronize(h->stream));
   h->stage = kCluster;
+  h->rr_dirty = true;  // the running view is grouped by node state
   h->shard_rank = 0;
   h->shard_n = 1;  // a new cluster: the partition -> rank table has to be set again
   return CRANE_OK;
@@ -769,88 +774,183 @@ int pending_append(crane_sched* h, const crane_pending_t* pd) {
   return CRANE_OK;
 }
 
-// The running table of this tick + the work and output buffers for the resident pending table.
-int set_running(crane_sched* h, const crane_running_t* rn) {
-  const uint32_t N = h->n_pending;
+// The rows of a host running table: the checks of crane_sched_running_append (`replace`:
+// the rows will replace the table rather than extend it)
+int running_check(crane_sched* h, const crane_running_t* rn, bool replace) {
   const uint32_t R = rn ? rn->n : 0;
-  if (R && (!rn->start_time || !rn->end_time || !rn->node_num || !rn->partition_priority || !rn->qos_priority ||
-            !rn->account || !rn->view_cpu_raw || !rn->view_mem))
+  if (!R) return CRANE_OK;
+  if (!rn->start_time || !rn->end_time || !rn->node_num || !rn->partition_priority || !rn->qos_priority ||
+      !rn->account || !rn->view_cpu_raw || !rn->view_mem)
     return fail(h, CRANE_EINVAL, "running: null column");
-  if (R) TRY(check_offsets(h, "running: alloc_off", rn->alloc_off, R));
-  uint32_t max_account = 0;
+  TRY(check_offsets(h, "running: alloc_off", rn->alloc_off, R));
+  const uint32_t E = rn->alloc_off[R];
+  if (E && (!rn->alloc_node || !rn->alloc_res)) return fail(h, CRANE_EINVAL, "running: null allocation table");
+  const uint64_t rows = replace ? 0 : h->n_rr, entries = replace ? 0 : h->h_rr_alloc_off.back();
+  if (rows + R > 0xfffffff0ull || entries + E > 0xfffffff0ull)
+    return fail(h, CRANE_EINVAL, "running: too many rows");
+  for (uint32_t j = 0; j < R; ++j) {
+    if (rn->account[j] > (1u << 24)) return fail(h, CRANE_EINVAL, "account ids must be dense (< 2^24)");
+    for (uint32_t k = rn->alloc_off[j]; k < rn->alloc_off[j + 1]; ++k)
+      if (rn->alloc_node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "running[%u]: node out of range", j);
+  }
+  return CRANE_OK;
+}
+
+void running_reset(crane_sched* h) {
+  h->n_rr = 0;
+  h->n_rr_dead = 0;
+  h->h_rr_alloc_off.assign(1, 0);
+  h->h_rr_account.clear();
+  h->h_rr_dead.clear();
+  h->rr_node_bound = 0;
+  h->rr_dirty = true;
+}
+
+// Appends the rows of a checked host running table to the resident table
+int running_append(crane_sched* h, const crane_running_t* rn) {
+  const uint32_t base = h->n_rr, R = rn ? rn->n : 0;
+  if (!R) return CRANE_OK;
+  const uint32_t eb = h->h_rr_alloc_off.back(), E = rn->alloc_off[R];
+  H2D_AT(h->d_rr_start, rn->start_time, base, R);
+  H2D_AT(h->d_rr_end, rn->end_time, base, R);
+  H2D_AT(h->d_rr_node_num, rn->node_num, base, R);
+  H2D_AT(h->d_rr_part_prio, rn->partition_priority, base, R);
+  H2D_AT(h->d_rr_qos_prio, rn->qos_priority, base, R);
+  H2D_AT(h->d_rr_account, rn->account, base, R);
+  H2D_AT(h->d_rr_cpu, rn->view_cpu_raw, base, R);
+  H2D_AT(h->d_rr_mem, rn->view_mem, base, R);
+  std::vector<uint32_t> no_resv(rn->reservation ? 0 : R, 0xffffffffu);
+  H2D_AT(h->d_rr_resv, rn->reservation ? rn->reservation : no_resv.data(), base, R);
+  std::vector<uint8_t> zeros(R, 0);
+  H2D_AT(h->d_rr_dead, zeros.data(), base, R);
+  for (uint32_t j = 0; j < R; ++j) {
+    h->h_rr_alloc_off.push_back(eb + rn->alloc_off[j + 1]);
+    h->h_rr_account.push_back(rn->account[j]);
+    h->h_rr_dead.push_back(0);
+  }
+  H2D_AT(h->d_rr_alloc_off, h->h_rr_alloc_off.data() + base, base, (size_t)R + 1);
+  H2D_AT(h->d_rr_alloc_node, rn->alloc_node, eb, E);
+  H2D_AT(h->d_rr_alloc_res, reinterpret_cast<const Row*>(rn->alloc_res), eb, E);
+  for (uint32_t k = 0; k < E; ++k) h->rr_node_bound = std::max(h->rr_node_bound, rn->alloc_node[k] + 1);
+  CU(cudaStreamSynchronize(h->stream));  // (the staging vectors are pageable)
+  h->n_rr = base + R;
+  h->rr_dirty = true;
+  return CRANE_OK;
+}
+
+RunTableDev run_table(crane_sched* h) {
+  RunTableDev rt{};
+  rt.n = h->n_rr;
+  rt.start_time = h->d_rr_start.p;
+  rt.end_time = h->d_rr_end.p;
+  rt.node_num = h->d_rr_node_num.p;
+  rt.partition_priority = h->d_rr_part_prio.p;
+  rt.qos_priority = h->d_rr_qos_prio.p;
+  rt.account = h->d_rr_account.p;
+  rt.reservation = h->d_rr_resv.p;
+  rt.view_cpu_raw = h->d_rr_cpu.p;
+  rt.view_mem = h->d_rr_mem.p;
+  rt.alloc_off = h->d_rr_alloc_off.p;
+  rt.alloc_node = h->d_rr_alloc_node.p;
+  rt.alloc_res = h->d_rr_alloc_res.p;
+  rt.dead = h->d_rr_dead.p;
+  return rt;
+}
+
+// The tick's RunningDev view of the live rows, on the device: the dense per-job columns
+// (live rows in row order), the allocations grouped by node state and the jobs grouped by
+// account, both stable (order inside a node state / account is row order, deviation D6).
+int regroup(crane_sched* h, uint32_t R, uint32_t max_rn_account) {
+  cudaStream_t st = h->stream;
+  const uint32_t Rt = h->n_rr, E = h->h_rr_alloc_off.back();
+  const RunTableDev rt = run_table(h);
+  CU(h->d_rn_start.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_end.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_node_num.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_part_prio.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_qos_prio.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_account.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_cpu.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_mem.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_acc_key.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_acc_job.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_slot_off.ensure((size_t)h->n_slots + 1));
+  CU(h->d_rn_slot_end.ensure(std::max<uint32_t>(E, 1)));
+  CU(h->d_rn_slot_res.ensure(std::max<uint32_t>(E, 1)));
+  CU(h->d_flag.ensure(1));
+  CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
+  uint64_t* keys;
+  uint32_t* vals;
+  // live rows in row order -> the dense columns (without tombstones: every row, in order)
+  if (R) {
+    vals = nullptr;
+    if (h->n_rr_dead) {
+      CRANE_LAUNCH(k_rt_live_keys, (Rt + 255) / 256, 256, 0, st, rt.dead, Rt, h->d_keys_a.p, h->d_vals_a.p);
+      TRY(radix_sort(h, Rt, 8, &keys, &vals));
+    }
+    const RunningCols o{h->d_rn_start.p, h->d_rn_end.p, h->d_rn_node_num.p, h->d_rn_part_prio.p,
+                        h->d_rn_qos_prio.p, h->d_rn_account.p, h->d_rn_cpu.p, h->d_rn_mem.p};
+    CRANE_LAUNCH(k_rt_gather, (R + 255) / 256, 256, 0, st, rt, vals, R, o);
+  }
+  // allocations by node state: stable sort of the entries (row order) by slot
+  if (E) {
+    NodeStateMap m{h->n_nodes, h->n_slots, h->n_comp, h->n_resv, h->d_node_slot.p, h->d_part_base.p, h->d_r_node_off.p, h->d_r_node.p};
+    const uint32_t nb = std::min<uint32_t>((Rt + 7) / 8, 8 * h->n_sm);
+    CRANE_LAUNCH(k_rt_entry_keys, nb, 256, 0, st, rt, m, h->d_keys_a.p, h->d_vals_a.p, h->d_flag.p);
+    int bits = 8;
+    while ((1ull << bits) <= (uint64_t)h->n_slots) bits += 8;
+    TRY(radix_sort(h, E, bits, &keys, &vals));
+    CRANE_LAUNCH(k_rt_offsets, (h->n_slots + 1 + 255) / 256, 256, 0, st, keys, E, h->n_slots, h->d_rn_slot_off.p);
+    CRANE_LAUNCH(k_rt_slot_gather, (E + 255) / 256, 256, 0, st, rt, keys, vals, E, h->d_rn_slot_off.p + h->n_slots,
+                 h->d_rn_slot_end.p, h->d_rn_slot_res.p);
+  } else {
+    CU(cudaMemsetAsync(h->d_rn_slot_off.p, 0, sizeof(uint32_t) * ((size_t)h->n_slots + 1), st));
+  }
+  // jobs by account: stable sort of the view's jobs by account
+  if (R) {
+    CRANE_LAUNCH(k_rt_acc_keys, (R + 255) / 256, 256, 0, st, h->d_rn_account.p, R, h->d_keys_a.p, h->d_vals_a.p);
+    int bits = 8;
+    while ((1ull << bits) <= (uint64_t)max_rn_account) bits += 8;
+    TRY(radix_sort(h, R, bits, &keys, &vals));
+    CU(cudaMemcpyAsync(h->d_rn_acc_key.p, keys, sizeof(uint64_t) * R, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(h->d_rn_acc_job.p, vals, sizeof(uint32_t) * R, cudaMemcpyDeviceToDevice, st));
+  }
+  CU(cudaGetLastError());
+  // a cluster with fewer nodes than the rows name: one flag read back
+  if (E && h->rr_node_bound > h->n_nodes) {
+    uint32_t bad = 0;
+    CU(cudaMemcpyAsync(&bad, h->d_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (bad) return fail(h, CRANE_EINVAL, "running: node out of range");
+  }
+  h->rr_dirty = false;
+  return CRANE_OK;
+}
+
+// "The next run uses the running table as it stands on the device": the view of the
+// live rows (regrouped when the rows or the node-state layout changed) and the work and
+// output buffers for the resident pending table.
+int keep_running(crane_sched* h) {
+  cudaStream_t st = h->stream;
+  const uint32_t N = h->n_pending, Rt = h->n_rr, R = Rt - h->n_rr_dead;
+  const uint32_t E = h->h_rr_alloc_off.back();
+  uint32_t max_rn_account = 0, max_account = 0;
+  for (uint32_t r = 0; r < Rt; ++r)
+    if (!h->h_rr_dead[r]) max_rn_account = std::max(max_rn_account, h->h_rr_account[r]);
   for (uint32_t i = 0; i < N; ++i) max_account = std::max(max_account, h->h_pd_account[i]);
-  for (uint32_t k = 0; k < R; ++k) max_account = std::max(max_account, rn->account[k]);
-  if (max_account > (1u << 24)) return fail(h, CRANE_EINVAL, "account ids must be dense (< 2^24)");
+  max_account = std::max(max_account, max_rn_account);
   const uint32_t A = (N + R) ? max_account + 1 : 0;
 
-  // ---- running jobs: columns + regrouping by node slot and by account ------
-  // (flattening of RnJobInScheduler::allocated_res; order inside a node /
-  // account is input order, deviation D6)
-  std::vector<uint32_t> slot_off((size_t)h->n_slots + 1, 0), acc_off((size_t)A + 1, 0), acc_job(R);
-  std::vector<uint8_t> acc_present(std::max<uint32_t>(A, 1), 0);
-  std::vector<int64_t> slot_end;
-  std::vector<Row> slot_res;
-  for (uint32_t i = 0; i < N; ++i)
-    if (!h->h_dead[i]) acc_present[h->h_pd_account[i]] = 1;
-  if (R) {
-    const uint32_t E = rn->alloc_off[R];
-    if (E && (!rn->alloc_node || !rn->alloc_res)) return fail(h, CRANE_EINVAL, "running: null allocation table");
-    for (uint32_t j = 0; j < R; ++j) {
-      acc_present[rn->account[j]] = 1;
-      acc_off[rn->account[j] + 1]++;
-      for (uint32_t k = rn->alloc_off[j]; k < rn->alloc_off[j + 1]; ++k) {
-        uint32_t n = rn->alloc_node[k];
-        if (n >= h->n_nodes) return fail(h, CRANE_EINVAL, "running[%u]: node out of range", j);
-        uint32_t g = running_slot(h, rn, j, n);
-        if (g != 0xffffffffu) slot_off[g + 1]++;  // nodes outside node_state_map are ignored (JS.cpp:5719)
-      }
-    }
-    for (uint32_t g = 0; g < h->n_slots; ++g) slot_off[g + 1] += slot_off[g];
-    for (uint32_t a = 0; a < A; ++a) acc_off[a + 1] += acc_off[a];
-    slot_end.resize(slot_off[h->n_slots]);
-    slot_res.resize(slot_off[h->n_slots]);
-    std::vector<uint32_t> fill_s(slot_off.begin(), slot_off.end() - 1), fill_a(acc_off.begin(), acc_off.end() - 1);
-    for (uint32_t j = 0; j < R; ++j) {
-      acc_job[fill_a[rn->account[j]]++] = j;
-      for (uint32_t k = rn->alloc_off[j]; k < rn->alloc_off[j + 1]; ++k) {
-        uint32_t g = running_slot(h, rn, j, rn->alloc_node[k]);
-        if (g == 0xffffffffu) continue;
-        uint32_t dst = fill_s[g]++;
-        slot_end[dst] = rn->end_time[j];
-        slot_res[dst] = reinterpret_cast<const Row&>(rn->alloc_res[k]);
-      }
-    }
-    H2D(h->d_rn_start, rn->start_time, R);
-    H2D(h->d_rn_end, rn->end_time, R);
-    H2D(h->d_rn_node_num, rn->node_num, R);
-    H2D(h->d_rn_part_prio, rn->partition_priority, R);
-    H2D(h->d_rn_qos_prio, rn->qos_priority, R);
-    H2D(h->d_rn_account, rn->account, R);
-    H2D(h->d_rn_cpu, rn->view_cpu_raw, R);
-    H2D(h->d_rn_mem, rn->view_mem, R);
-    H2D(h->d_rn_slot_end, slot_end.data(), slot_end.size());
-    H2D(h->d_rn_slot_res, slot_res.data(), slot_res.size());
-  }
-  // always present: k_service / k_node_init index these even with no running job
-  H2D(h->d_rn_acc_off, acc_off.data(), acc_off.size());
-  H2D(h->d_rn_acc_job, acc_job.data(), acc_job.size());
-  H2D(h->d_rn_slot_off, slot_off.data(), slot_off.size());
-  H2D(h->d_acc_present, acc_present.data(), acc_present.size());
-  // staging vectors above are pageable: the copies have completed on return,
-  // but make it explicit before they go out of scope
-  CU(cudaStreamSynchronize(h->stream));
-  h->n_running = R;
-  h->n_accounts = A;
-
-  // ---- work + output buffers ----------------------------------------------
+  // ---- work + output buffers (the sorts of the regroup use the priority sort's) ----
   size_t n1 = std::max<uint32_t>(N, 1);
+  const size_t ns = std::max<size_t>({n1, (size_t)Rt, (size_t)E});
   CU(h->d_bounds.ensure(1));
   CU(h->d_acc_service.ensure(std::max<uint32_t>(A, 1)));
   CU(h->d_prio.ensure(n1));
-  CU(h->d_keys_a.ensure(n1));
-  CU(h->d_keys_b.ensure(n1));
-  CU(h->d_vals_a.ensure(n1));
-  CU(h->d_vals_b.ensure(n1));
+  CU(h->d_keys_a.ensure(ns));
+  CU(h->d_keys_b.ensure(ns));
+  CU(h->d_vals_a.ensure(ns));
+  CU(h->d_vals_b.ensure(ns));
   uint32_t nq = std::min<uint32_t>(N, h->cfg.scheduled_batch_size);
   CU(h->d_jobq.ensure(std::max<uint32_t>(nq, 1)));
   CU(h->d_bitmap.ensure((size_t)std::max<uint32_t>(nq, 1) * h->words_per_row));
@@ -863,7 +963,30 @@ int set_running(crane_sched* h, const crane_running_t* rn) {
   CU(h->d_out_node.ensure(ta));
   CU(h->d_out_ntasks.ensure(ta));
   CU(h->d_out_res.ensure(ta));
+
+  CU(cudaEventRecord(h->ev[kEvKeepBegin], st));
+  if (h->rr_dirty) TRY(regroup(h, R, max_rn_account));
+  // ---- accounts: offsets of the account groups, accounts present (pending included) ----
+  CU(h->d_rn_acc_off.ensure((size_t)A + 1));
+  CU(h->d_acc_present.ensure(std::max<uint32_t>(A, 1)));
+  CRANE_LAUNCH(k_rt_offsets, (A + 1 + 255) / 256, 256, 0, st, h->d_rn_acc_key.p, R, A, h->d_rn_acc_off.p);
+  CU(cudaMemsetAsync(h->d_acc_present.p, 0, std::max<uint32_t>(A, 1), st));
+  if (N + R)
+    CRANE_LAUNCH(k_acc_present, (N + R + 255) / 256, 256, 0, st, h->d_account.p, h->n_dead ? h->d_dead.p : nullptr, N,
+                 h->d_rn_account.p, R, h->d_acc_present.p);
+  CU(cudaEventRecord(h->ev[kEvKeepEnd], st));
+  CU(cudaGetLastError());
+  h->n_running = R;
+  h->n_accounts = A;
   return CRANE_OK;
+}
+
+// The running table of this tick from a host table: reset + append + keep_running
+int set_running(crane_sched* h, const crane_running_t* rn) {
+  TRY(running_check(h, rn, true));
+  running_reset(h);
+  TRY(running_append(h, rn));
+  return keep_running(h);
 }
 
 }  // namespace
@@ -908,6 +1031,140 @@ int crane_sched_pending_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n
   CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, h->stream, h->d_erase_rows.p, n, h->d_dead.p);
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(h->stream));
+  return CRANE_OK;
+}
+
+uint32_t crane_sched_running_rows(const crane_sched_t* h) { return h ? h->n_rr : 0; }
+
+int crane_sched_running_append(crane_sched_t* h, const crane_running_t* rows, uint32_t* first_row) {
+  if (!h || !rows) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "running_append"));
+  CU(cudaSetDevice(h->device));
+  TRY(running_check(h, rows, false));
+  lower_stage(h, kCluster);  // the next run needs crane_sched_keep_running
+  const uint32_t base = h->n_rr;
+  TRY(running_append(h, rows));
+  if (first_row) *first_row = base;
+  return CRANE_OK;
+}
+
+int crane_sched_running_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n) {
+  if (!h || (n && !rows)) return CRANE_EINVAL;
+  CU(cudaSetDevice(h->device));
+  for (uint32_t k = 0; k < n; ++k)
+    if (rows[k] >= h->n_rr) return fail(h, CRANE_EINVAL, "running_erase: row %u out of range", rows[k]);
+  lower_stage(h, kCluster);
+  if (!n) return CRANE_OK;
+  for (uint32_t k = 0; k < n; ++k)
+    if (!h->h_rr_dead[rows[k]]) { h->h_rr_dead[rows[k]] = 1; h->n_rr_dead++; }
+  H2D(h->d_erase_rows, rows, n);
+  CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, h->stream, h->d_erase_rows.p, n, h->d_rr_dead.p);
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(h->stream));
+  h->rr_dirty = true;
+  return CRANE_OK;
+}
+
+int crane_sched_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32_t* first_row) {
+  if (!h || (n && !rows)) return CRANE_EINVAL;
+  if (h->shard_n > 1)  // other ranks' placement columns are zero until the caller's all-reduce
+    return fail(h, CRANE_ENOSYS, "start: not available on a sharded handle (set_shard n_ranks > 1)");
+  TRY(require(h, kRan, "start"));
+  CU(cudaSetDevice(h->device));
+  cudaStream_t st = h->stream;
+  const uint32_t base = h->n_rr, eb = h->h_rr_alloc_off.back();
+  {
+    std::vector<uint32_t> sorted(rows, rows + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint32_t k = 0; k < n; ++k) {
+      if (sorted[k] >= h->n_pending) return fail(h, CRANE_EINVAL, "start: row %u out of range", sorted[k]);
+      if (h->h_dead[sorted[k]]) return fail(h, CRANE_EINVAL, "start: row %u was erased", sorted[k]);
+      if (k && sorted[k] == sorted[k - 1]) return fail(h, CRANE_EINVAL, "start: row %u listed twice", sorted[k]);
+    }
+  }
+  // the new rows' allocation offsets: node_num of the started rows (host mirror of alloc_off)
+  std::vector<uint32_t> off(n + 1, eb);
+  for (uint32_t k = 0; k < n; ++k) {
+    const uint64_t e = (uint64_t)off[k] + (h->h_alloc_off[rows[k] + 1] - h->h_alloc_off[rows[k]]);
+    if (e > 0xfffffff0ull || (uint64_t)base + n > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "start: too many running rows");
+    off[k + 1] = (uint32_t)e;
+  }
+  if (n) {
+    // every row must hold a start-now placement of the last run (after any qos_filter)
+    H2D(h->d_start_rows, rows, n);
+    CU(h->d_flag.ensure(1));
+    CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
+    CRANE_LAUNCH(k_start_check, (n + 255) / 256, 256, 0, st, h->d_start_rows.p, n, h->d_reason.p, h->d_flag.p);
+    uint32_t bad = 0;
+    CU(cudaMemcpyAsync(&bad, h->d_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    if (bad) return fail(h, CRANE_EINVAL, "start: a row does not hold a start-now placement of the last run");
+  }
+  lower_stage(h, kCluster);  // the run's outputs are void from here on
+  if (!n) {
+    if (first_row) *first_row = base;
+    return CRANE_OK;
+  }
+  const uint32_t rows_end = base + n, ent_end = off[n];
+  CU(h->d_rr_start.grow(rows_end, base, st));
+  CU(h->d_rr_end.grow(rows_end, base, st));
+  CU(h->d_rr_node_num.grow(rows_end, base, st));
+  CU(h->d_rr_part_prio.grow(rows_end, base, st));
+  CU(h->d_rr_qos_prio.grow(rows_end, base, st));
+  CU(h->d_rr_account.grow(rows_end, base, st));
+  CU(h->d_rr_resv.grow(rows_end, base, st));
+  CU(h->d_rr_cpu.grow(rows_end, base, st));
+  CU(h->d_rr_mem.grow(rows_end, base, st));
+  CU(h->d_rr_alloc_node.grow(ent_end, eb, st));
+  CU(h->d_rr_alloc_res.grow(ent_end, eb, st));
+  H2D_AT(h->d_rr_alloc_off, off.data(), base, (size_t)n + 1);
+  std::vector<uint8_t> zeros(n, 0);
+  H2D_AT(h->d_rr_dead, zeros.data(), base, n);
+  PendingDev pd{};
+  pd.node_num = h->d_node_num.p;
+  pd.alloc_off = h->d_alloc_off.p;
+  pd.partition_priority = h->d_part_prio.p;
+  pd.qos_priority = h->d_qos_prio.p;
+  pd.account = h->d_account.p;
+  pd.reservation = h->have_pd_resv ? h->d_pd_resv.p : nullptr;
+  PlaceDev out{};
+  out.start_time = h->d_out_start.p;
+  out.end_time = h->d_out_end.p;
+  out.alloc_node = h->d_out_node.p;
+  out.alloc_res = h->d_out_res.p;
+  RunTableDev rt = run_table(h);
+  const uint32_t nb = std::min<uint32_t>((n + 7) / 8, 8 * h->n_sm);
+  CRANE_LAUNCH(k_start, nb, 256, 0, st, pd, out, h->d_start_rows.p, n, base, rt);
+  // the pending rows leave the pending table (m_pending_job_map_.erase, JobScheduler.cpp:1305)
+  CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, st, h->d_start_rows.p, n, h->d_dead.p);
+  CU(cudaGetLastError());
+  for (uint32_t k = 0; k < n; ++k) {
+    h->h_dead[rows[k]] = 1;
+    h->h_rr_account.push_back(h->h_pd_account[rows[k]]);
+    h->h_rr_dead.push_back(0);
+    h->h_rr_alloc_off.push_back(off[k + 1]);
+  }
+  h->n_dead += n;
+  h->n_rr = rows_end;
+  h->rr_node_bound = std::max(h->rr_node_bound, h->n_nodes);  // (placements are on this cluster's nodes)
+  h->rr_dirty = true;
+  CU(cudaStreamSynchronize(st));
+  if (first_row) *first_row = base;
+  return CRANE_OK;
+}
+
+int crane_sched_keep_running(crane_sched_t* h, float* device_ms) {
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "keep_running"));
+  CU(cudaSetDevice(h->device));
+  lower_stage(h, kCluster);
+  TRY(keep_running(h));
+  if (device_ms) {
+    CU(cudaEventSynchronize(h->ev[kEvKeepEnd]));
+    *device_ms = elapsed_ms(h, kEvKeepBegin, kEvKeepEnd);
+  }
+  h->stage = kUploaded;
   return CRANE_OK;
 }
 

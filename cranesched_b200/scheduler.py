@@ -73,6 +73,16 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.crane_sched_set_running.argtypes = [C.c_void_p, P(abi.RunningC)]
     lib.crane_sched_pending_rows.restype = C.c_uint32
     lib.crane_sched_pending_rows.argtypes = [C.c_void_p]
+    lib.crane_sched_running_append.restype = C.c_int
+    lib.crane_sched_running_append.argtypes = [C.c_void_p, P(abi.RunningC), P(C.c_uint32)]
+    lib.crane_sched_running_erase.restype = C.c_int
+    lib.crane_sched_running_erase.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    lib.crane_sched_start.restype = C.c_int
+    lib.crane_sched_start.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, P(C.c_uint32)]
+    lib.crane_sched_keep_running.restype = C.c_int
+    lib.crane_sched_keep_running.argtypes = [C.c_void_p, P(C.c_float)]
+    lib.crane_sched_running_rows.restype = C.c_uint32
+    lib.crane_sched_running_rows.argtypes = [C.c_void_p]
     lib.crane_sched_set_shard.restype = C.c_int
     lib.crane_sched_set_shard.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
     lib.crane_sched_device_placements.restype = C.c_int
@@ -90,7 +100,8 @@ def load_library(path: str | None = None) -> C.CDLL:
 
 EXPORTS = ("crane_sched_create", "crane_sched_destroy", "crane_sched_last_error",
            "crane_sched_set_cluster", "crane_sched_set_reservations", "crane_sched_node_select", "crane_sched_upload", "crane_sched_pending_reset", "crane_sched_pending_append", "crane_sched_pending_erase",
-           "crane_sched_set_running", "crane_sched_pending_rows",
+           "crane_sched_set_running", "crane_sched_pending_rows", "crane_sched_running_append",
+           "crane_sched_running_erase", "crane_sched_start", "crane_sched_keep_running", "crane_sched_running_rows",
            "crane_sched_run", "crane_sched_fetch", "crane_sched_sync", "crane_sched_get_timing",
            "crane_sched_qos_filter", "crane_sched_set_shard", "crane_sched_device_placements",
            "crane_sched_debug_bitmap", "crane_sched_debug_profile", "crane_sched_schedule_steps")
@@ -168,6 +179,37 @@ class GpuScheduler:
 
     def pending_rows(self) -> int:
         return int(self._lib.crane_sched_pending_rows(self._h))
+
+    # --- the running table resident on the device across ticks ----------------------
+    def running_append(self, rows: abi.Running) -> int:
+        """Running jobs from the host (recovery, jobs started elsewhere): returns the
+        index of the first new row."""
+        c, first = rows.as_c(), C.c_uint32(0)
+        self._check(self._lib.crane_sched_running_append(self._h, C.byref(c), C.byref(first)))
+        return first.value
+
+    def running_erase(self, rows):
+        """Jobs that ended or were cancelled (FreeResourceFromNode): their rows become tombstones."""
+        r = np.ascontiguousarray(rows, np.uint32)
+        self._check(self._lib.crane_sched_running_erase(self._h, r.ctypes.data, len(r)))
+
+    def start(self, pending_rows) -> int:
+        """Moves pending rows the last run starts now into the running table, on the device
+        (JobScheduler.cpp:1273-1305); returns the running row of the first one."""
+        r = np.ascontiguousarray(pending_rows, np.uint32)
+        first = C.c_uint32(0)
+        self._check(self._lib.crane_sched_start(self._h, r.ctypes.data, len(r), C.byref(first)))
+        return first.value
+
+    def keep_running(self) -> float:
+        """The next run uses the running table as it stands on the device; returns the
+        device ms of the regroup."""
+        ms = C.c_float(0.0)
+        self._check(self._lib.crane_sched_keep_running(self._h, C.byref(ms)))
+        return ms.value
+
+    def running_rows(self) -> int:
+        return int(self._lib.crane_sched_running_rows(self._h))
 
     def run(self, now: int):
         self._check(self._lib.crane_sched_run(self._h, now))

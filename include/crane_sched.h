@@ -292,6 +292,42 @@ int crane_sched_pending_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n
 int crane_sched_set_running(crane_sched_t* h, const crane_running_t* running);
 uint32_t crane_sched_pending_rows(const crane_sched_t* h);
 
+/* The running table kept resident on the device across ticks. Rows keep their
+ * index until the table is replaced; an erased row is a tombstone that takes part
+ * in nothing (timelines, initial cost, priority bounds, fair-share service).
+ * A steady-state tick is
+ *     crane_sched_start(h, started, n, &first);    after the previous run
+ *     crane_sched_running_erase(h, ended, m);
+ *     crane_sched_keep_running(h, NULL); crane_sched_run(h, now); crane_sched_fetch(h, out)
+ * and uploads no job data. crane_sched_set_running == reset; running_append;
+ * keep_running, which is also how a caller compacts the tombstones. Reservation
+ * indices of running rows follow crane_sched_set_reservations, as for pending rows.
+ *
+ * running_append: appends host rows (recovery at daemon start, jobs started
+ *   elsewhere), checked as set_running checks them; *first_row (optional) = the
+ *   index of the first new row.
+ * running_erase: a job ended or was cancelled (CranedMetaContainer FreeResourceFromNode).
+ * start: moves the given pending rows into the running table on the device, from
+ *   the last run's placements (JobScheduler.cpp:1273-1305): start / end time from the
+ *   placement; node_num, partition_priority, qos_priority, account and reservation
+ *   from the pending row; the allocation rows are the job's placement rows; the
+ *   view is their sum. New rows follow the order of `pending_rows`; the pending rows
+ *   are then erased. CRANE_EINVAL for a row out of range, erased, listed twice, or
+ *   whose reason after the last run (and any crane_sched_qos_filter) is not
+ *   CRANE_REASON_NONE. Needs a completed run and voids its outputs. CRANE_ENOSYS on a
+ *   sharded handle (set_shard n_ranks > 1).
+ * keep_running: the next run uses the running table as it stands on the device.
+ *   Builds the run's view of the live rows (regrouped only when the rows or the
+ *   cluster / reservation layout changed) and sizes the work buffers for the current
+ *   pending table; then crane_sched_run may be called. Allocations on nodes outside
+ *   the node states are ignored (JobScheduler.cpp:5719); a node index >= n_nodes is
+ *   CRANE_EINVAL. *device_ms (optional) receives the CUDA-event time of its kernels. */
+int crane_sched_running_append(crane_sched_t* h, const crane_running_t* rows, uint32_t* first_row);
+int crane_sched_running_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n);
+int crane_sched_start(crane_sched_t* h, const uint32_t* pending_rows, uint32_t n, uint32_t* first_row);
+int crane_sched_keep_running(crane_sched_t* h, float* device_ms);
+uint32_t crane_sched_running_rows(const crane_sched_t* h);
+
 /* Blocks until the handle's stream is idle; *run_ms (optional) receives the
  * device time of the last crane_sched_run (CUDA events on that stream). */
 int crane_sched_sync(crane_sched_t* h, float* run_ms);
