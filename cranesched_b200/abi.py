@@ -29,6 +29,10 @@ REASON_RESOURCE = 2
 REASON_RESERVED = 3
 REASON_PART_NOT_FOUND = 4
 REASON_RESV_NOT_FOUND = 5
+REASON_HELD = 7
+REASON_BEGIN_TIME = 8
+REASON_DEPENDENCY = 9
+REASON_DEPENDENCY_NEVER = 10
 REASON_ERASED = 255  # a row removed from the device-resident pending table
 REASON_QOS_CPU = 16
 REASON_QOS_JOBS = 17
@@ -42,6 +46,10 @@ REASON_STR = {
     2: "Resource",
     3: "Resource Reserved",
     4: "Partition Not Found",
+    7: "Held",
+    8: "BeginTime",
+    9: "Dependency",
+    10: "DependencyNeverSatisfied",
     16: "QosCpuResourceLimit",
     17: "QosJobsResourceLimit",
     18: "QosWallTimeLimit",
@@ -667,6 +675,65 @@ class Reservations:
     def as_c(self) -> ReservationsC:
         return ReservationsC(self.n, _ptr(self.start_time), _ptr(self.end_time), _ptr(self.node_off),
                              _ptr(self.node), _ptr(self.res))
+
+
+# ---------------------------------------------------------------------------
+# The gate of the resident pending table: hold, begin time, dependencies
+# ---------------------------------------------------------------------------
+TIME_PAST = -(2 ** 63)     # absl::InfinitePast
+TIME_FUTURE = 2 ** 63 - 1  # absl::InfiniteFuture
+DEP_AFTER, DEP_AFTER_ANY, DEP_AFTER_OK, DEP_AFTER_NOT_OK = 0, 1, 2, 3  # DependencyType (PublicDefs.proto:136-141)
+DEPENDEE_PENDING, DEPENDEE_RUNNING, DEPENDEE_EVENT = 0, 1, 2
+
+
+class DependenciesC(C.Structure):
+    """crane_dependencies_t"""
+    _fields_ = [("n", C.c_uint32), ("row", _p), ("is_or", _p), ("dep_off", _p), ("kind", _p), ("dependee", _p),
+                ("type", _p), ("delay_s", _p), ("event_time", _p)]
+
+
+@dataclass
+class Dependencies:
+    """Dependency lists of pending rows: row k is pending row `row[k]`, its entries are
+    [dep_off[k], dep_off[k+1]) of (kind, dependee row, type, delay, event time)."""
+    row: np.ndarray
+    is_or: np.ndarray
+    dep_off: np.ndarray
+    kind: np.ndarray
+    dependee: np.ndarray
+    type: np.ndarray
+    delay_s: np.ndarray
+    event_time: np.ndarray
+
+    def __post_init__(self):
+        n = len(self.row)
+        self.row = _arr(self.row, np.uint32, n)
+        self.is_or = _arr(self.is_or, np.uint8, n)
+        self.dep_off = _arr(self.dep_off, np.uint32, n + 1)
+        m = int(self.dep_off[-1])
+        self.kind = _arr(self.kind, np.uint8, m)
+        self.dependee = _arr(self.dependee, np.uint32, m)
+        self.type = _arr(self.type, np.uint8, m)
+        self.delay_s = _arr(self.delay_s, np.uint64, m)
+        self.event_time = _arr(self.event_time, np.int64, m)
+
+    @staticmethod
+    def from_lists(rows, is_or, entries) -> "Dependencies":
+        """entries[k] = list of (kind, dependee, type, delay_s, event_time) of rows[k]."""
+        off = np.zeros(len(rows) + 1, np.uint32)
+        off[1:] = np.cumsum([len(e) for e in entries]) if len(entries) else []
+        flat = [x for e in entries for x in e]
+        col = lambda i, dt: np.array([x[i] for x in flat], dt)  # noqa: E731
+        return Dependencies(rows, is_or, off, col(0, np.uint8), col(1, np.uint32), col(2, np.uint8),
+                            col(3, np.uint64), col(4, np.int64))
+
+    @property
+    def n(self):
+        return len(self.row)
+
+    def as_c(self) -> DependenciesC:
+        return DependenciesC(self.n, _ptr(self.row), _ptr(self.is_or), _ptr(self.dep_off), _ptr(self.kind),
+                             _ptr(self.dependee), _ptr(self.type), _ptr(self.delay_s), _ptr(self.event_time))
 
 
 # ---------------------------------------------------------------------------

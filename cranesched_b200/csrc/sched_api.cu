@@ -31,6 +31,7 @@
 #include "qos_kernels.cuh"
 #include "step_kernels.cuh"
 #include "running_kernels.cuh"
+#include "gate_kernels.cuh"
 
 using namespace crane;
 
@@ -179,6 +180,21 @@ struct crane_sched {
   DBuf<uint64_t> d_rn_mem, d_rn_acc_key;
   DBuf<Row> d_rn_slot_res;
   DBuf<uint8_t> d_acc_present;
+  // the gate of the pending table (gate_kernels.cuh): off until a gate call after pending_reset
+  bool gate_on = false;
+  uint32_t gate_n = 0;              // rows [0, gate_n) have gate state
+  std::vector<uint8_t> h_has_deps;  // [gate_n] the row got its dependency list
+  uint32_t n_ent = 0;               // dependency entries, live or retired
+  DBuf<uint8_t> d_g_held, d_g_is_or, d_g_code;
+  DBuf<int64_t> d_g_begin;
+  DBuf<long long> d_g_ready;
+  DBuf<uint32_t> d_g_open;
+  DBuf<uint32_t> d_e_dependent, d_e_dependee;
+  DBuf<uint8_t> d_e_kind, d_e_type, d_e_live;
+  DBuf<uint64_t> d_e_delay;
+  DBuf<uint32_t> d_ev_rows, d_ev_u32;  // per call: sorted rows + their positions | exit codes, offsets
+  DBuf<int64_t> d_ev_i64;              // per call: end / event times, begin times
+  DBuf<uint8_t> d_ev_u8;               // per call: held, is_or
   // work buffers
   DBuf<Bounds> d_bounds;
   DBuf<double> d_acc_service, d_prio;
@@ -989,6 +1005,69 @@ int set_running(crane_sched* h, const crane_running_t* rn) {
   return keep_running(h);
 }
 
+GateDev gate_dev(crane_sched* h) {
+  GateDev g{};
+  g.n = h->gate_n;
+  g.dead = h->n_dead ? h->d_dead.p : nullptr;
+  g.held = h->d_g_held.p;
+  g.begin = h->d_g_begin.p;
+  g.is_or = h->d_g_is_or.p;
+  g.open = h->d_g_open.p;
+  g.ready = h->d_g_ready.p;
+  g.n_ent = h->n_ent;
+  g.dependent = h->d_e_dependent.p;
+  g.dependee = h->d_e_dependee.p;
+  g.kind = h->d_e_kind.p;
+  g.type = h->d_e_type.p;
+  g.live = h->d_e_live.p;
+  g.delay = h->d_e_delay.p;
+  return g;
+}
+
+// Turns the gate on and gives the rows appended since the last gate call their state:
+// not held, beginning at InfinitePast, no dependencies
+int gate_fit(crane_sched* h) {
+  h->gate_on = true;
+  const uint32_t from = h->gate_n, to = h->n_pending;
+  if (to <= from) return CRANE_OK;
+  cudaStream_t st = h->stream;
+  CU(h->d_g_held.grow(to, from, st));
+  CU(h->d_g_begin.grow(to, from, st));
+  CU(h->d_g_is_or.grow(to, from, st));
+  CU(h->d_g_open.grow(to, from, st));
+  CU(h->d_g_ready.grow(to, from, st));
+  h->gate_n = to;
+  h->h_has_deps.resize(to, 0);
+  CRANE_LAUNCH(k_gate_init, (to - from + 255) / 256, 256, 0, st, gate_dev(h), from, to);
+  CU(cudaGetLastError());
+  return CRANE_OK;
+}
+
+// The rows of a call on the device, sorted, followed by their places in the call's list
+int upload_call_rows(crane_sched* h, const uint32_t* rows, uint32_t n) {
+  std::vector<uint32_t> idx(n), buf(2 * (size_t)n);
+  for (uint32_t k = 0; k < n; ++k) idx[k] = k;
+  std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return rows[a] < rows[b]; });
+  for (uint32_t k = 0; k < n; ++k) {
+    buf[k] = rows[idx[k]];
+    buf[n + k] = idx[k];
+  }
+  H2D(h->d_ev_rows, buf.data(), buf.size());
+  CU(cudaStreamSynchronize(h->stream));  // (buf is pageable)
+  return CRANE_OK;
+}
+
+// k_dep_fire over `threads` entries for the events of the call whose rows upload_call_rows placed
+int dep_fire(crane_sched* h, DepEvents ev, uint32_t n_rows, uint32_t threads) {
+  if (!threads) return CRANE_OK;
+  ev.n = n_rows;
+  ev.rows = h->d_ev_rows.p;
+  ev.pos = h->d_ev_rows.p + n_rows;
+  CRANE_LAUNCH(k_dep_fire, (threads + 255) / 256, 256, 0, h->stream, gate_dev(h), ev);
+  CU(cudaGetLastError());
+  return CRANE_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1003,6 +1082,10 @@ int crane_sched_pending_reset(crane_sched_t* h) {
   h->h_alloc_off.assign(1, 0);
   h->h_pd_account.clear();
   h->h_dead.clear();
+  h->gate_on = false;
+  h->gate_n = 0;
+  h->h_has_deps.clear();
+  h->n_ent = 0;
   lower_stage(h, kCluster);
   return CRANE_OK;
 }
@@ -1139,6 +1222,14 @@ int crane_sched_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32
   // the pending rows leave the pending table (m_pending_job_map_.erase, JobScheduler.cpp:1305)
   CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, st, h->d_start_rows.p, n, h->d_dead.p);
   CU(cudaGetLastError());
+  if (h->n_ent) {  // AFTER fires at the placement's start (JobScheduler.cpp:1549), the rest follow the job
+    TRY(upload_call_rows(h, rows, n));
+    DepEvents ev{};
+    ev.mode = kFireStart;
+    ev.time = h->d_out_start.p;
+    ev.base = base;
+    TRY(dep_fire(h, ev, n, h->n_ent));
+  }
   for (uint32_t k = 0; k < n; ++k) {
     h->h_dead[rows[k]] = 1;
     h->h_rr_account.push_back(h->h_pd_account[rows[k]]);
@@ -1151,6 +1242,134 @@ int crane_sched_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32
   h->rr_dirty = true;
   CU(cudaStreamSynchronize(st));
   if (first_row) *first_row = base;
+  return CRANE_OK;
+}
+
+int crane_sched_pending_set_gate(crane_sched_t* h, const uint32_t* rows, uint32_t n, const uint8_t* held,
+                                 const int64_t* begin_time) {
+  if (!h || (n && !rows)) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "pending_set_gate"));
+  CU(cudaSetDevice(h->device));
+  for (uint32_t k = 0; k < n; ++k)
+    if (rows[k] >= h->n_pending) return fail(h, CRANE_EINVAL, "pending_set_gate: row %u out of range", rows[k]);
+  lower_stage(h, kCluster);
+  TRY(gate_fit(h));
+  if (n && (held || begin_time)) {
+    H2D(h->d_ev_rows, rows, n);
+    if (held) H2D(h->d_ev_u8, held, n);
+    if (begin_time) H2D(h->d_ev_i64, begin_time, n);
+    CRANE_LAUNCH(k_gate_set, (n + 255) / 256, 256, 0, h->stream, gate_dev(h), h->d_ev_rows.p, n,
+                 held ? h->d_ev_u8.p : nullptr, begin_time ? h->d_ev_i64.p : nullptr);
+    CU(cudaGetLastError());
+  }
+  CU(cudaStreamSynchronize(h->stream));
+  return CRANE_OK;
+}
+
+int crane_sched_pending_depend(crane_sched_t* h, const crane_dependencies_t* d) {
+  if (!h || !d) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "pending_depend"));
+  CU(cudaSetDevice(h->device));
+  const uint32_t n = d->n;
+  if (n && (!d->row || !d->is_or)) return fail(h, CRANE_EINVAL, "depend: null column");
+  TRY(check_offsets(h, "depend: dep_off", d->dep_off, n));
+  const uint32_t m = d->dep_off[n];
+  if (m && (!d->kind || !d->dependee || !d->type || !d->delay_s)) return fail(h, CRANE_EINVAL, "depend: null entry column");
+  if ((uint64_t)h->n_ent + m > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "depend: too many entries");
+  {
+    std::vector<uint32_t> sorted(d->row, d->row + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint32_t k = 1; k < n; ++k)
+      if (sorted[k] == sorted[k - 1]) return fail(h, CRANE_EINVAL, "depend: row %u listed twice", sorted[k]);
+  }
+  std::vector<uint32_t> dependent(m), dependee(m);
+  for (uint32_t k = 0; k < n; ++k) {
+    const uint32_t r = d->row[k];
+    if (r >= h->n_pending) return fail(h, CRANE_EINVAL, "depend: row %u out of range", r);
+    if (h->h_dead[r]) return fail(h, CRANE_EINVAL, "depend: row %u was erased", r);
+    if (r < h->h_has_deps.size() && h->h_has_deps[r]) return fail(h, CRANE_EINVAL, "depend: row %u already has its list", r);
+    for (uint32_t e = d->dep_off[k]; e < d->dep_off[k + 1]; ++e) {
+      const uint8_t kind = d->kind[e];
+      const uint32_t q = d->dependee[e];
+      if (kind > CRANE_DEPENDEE_EVENT) return fail(h, CRANE_EINVAL, "depend: row %u: dependee kind %u", r, kind);
+      if (d->type[e] > CRANE_DEP_AFTER_NOT_OK) return fail(h, CRANE_EINVAL, "depend: row %u: type %u", r, d->type[e]);
+      if (d->delay_s[e] >= (1ull << 62)) return fail(h, CRANE_EINVAL, "depend: row %u: delay out of range", r);
+      if (kind == CRANE_DEPENDEE_EVENT) {
+        if (!d->event_time) return fail(h, CRANE_EINVAL, "depend: EVENT entries without event_time");
+      } else if (kind == CRANE_DEPENDEE_PENDING) {
+        if (q >= h->n_pending || h->h_dead[q]) return fail(h, CRANE_EINVAL, "depend: row %u: pending dependee %u missing", r, q);
+        if (q == r) return fail(h, CRANE_EINVAL, "depend: row %u depends on itself", r);
+      } else if (q >= h->n_rr || h->h_rr_dead[q]) {
+        return fail(h, CRANE_EINVAL, "depend: row %u: running dependee %u missing", r, q);
+      }
+      for (uint32_t e2 = d->dep_off[k]; e2 < e && kind != CRANE_DEPENDEE_EVENT; ++e2)  // `deps` is a map
+        if (d->kind[e2] == kind && d->dependee[e2] == q) return fail(h, CRANE_EINVAL, "depend: row %u lists a dependee twice", r);
+      dependent[e] = r;
+      dependee[e] = kind == CRANE_DEPENDEE_EVENT ? 0 : q;
+    }
+  }
+  lower_stage(h, kCluster);
+  TRY(gate_fit(h));
+  cudaStream_t st = h->stream;
+  const uint32_t e0 = h->n_ent;
+  if (m) {
+    std::vector<uint8_t> live(m, 1);
+    H2D_AT(h->d_e_dependent, dependent.data(), e0, m);
+    H2D_AT(h->d_e_dependee, dependee.data(), e0, m);
+    H2D_AT(h->d_e_kind, d->kind, e0, m);
+    H2D_AT(h->d_e_type, d->type, e0, m);
+    H2D_AT(h->d_e_delay, d->delay_s, e0, m);
+    H2D_AT(h->d_e_live, live.data(), e0, m);
+    if (d->event_time) H2D(h->d_ev_i64, d->event_time, m);
+    CU(cudaStreamSynchronize(st));  // (the staging vectors are pageable)
+  }
+  h->n_ent = e0 + m;
+  if (n) {
+    H2D(h->d_ev_rows, d->row, n);
+    H2D(h->d_ev_u8, d->is_or, n);
+    H2D(h->d_ev_u32, d->dep_off, (size_t)n + 1);
+    CRANE_LAUNCH(k_dep_rows, (n + 255) / 256, 256, 0, st, gate_dev(h), h->d_ev_rows.p, n, h->d_ev_u8.p, h->d_ev_u32.p);
+    CU(cudaGetLastError());
+  }
+  // entries resolved on arrival: EVENT, and AFTER on a running dependee
+  DepEvents ev{};
+  ev.mode = kFireDepend;
+  ev.run_start = h->d_rr_start.p;
+  ev.event_time = d->event_time ? h->d_ev_i64.p : nullptr;
+  ev.e0 = e0;
+  TRY(dep_fire(h, ev, 0, m));
+  for (uint32_t k = 0; k < n; ++k) h->h_has_deps[d->row[k]] = 1;
+  CU(cudaStreamSynchronize(st));
+  return CRANE_OK;
+}
+
+int crane_sched_pending_cancel(crane_sched_t* h, const uint32_t* rows, uint32_t n, int64_t cancel_time) {
+  TRY(crane_sched_pending_erase(h, rows, n));
+  if (!n || !h->n_ent) return CRANE_OK;
+  TRY(upload_call_rows(h, rows, n));
+  DepEvents ev{};
+  ev.mode = kFireCancel;
+  ev.t = cancel_time;
+  TRY(dep_fire(h, ev, n, h->n_ent));
+  CU(cudaStreamSynchronize(h->stream));
+  return CRANE_OK;
+}
+
+int crane_sched_running_end(crane_sched_t* h, const uint32_t* rows, uint32_t n, const int64_t* end_time,
+                            const uint32_t* exit_code) {
+  if (!h) return CRANE_EINVAL;
+  if (n && (!end_time || !exit_code)) return fail(h, CRANE_EINVAL, "running_end: null column");
+  TRY(crane_sched_running_erase(h, rows, n));
+  if (!n || !h->n_ent) return CRANE_OK;
+  TRY(upload_call_rows(h, rows, n));
+  H2D(h->d_ev_i64, end_time, n);
+  H2D(h->d_ev_u32, exit_code, n);
+  DepEvents ev{};
+  ev.mode = kFireEnd;
+  ev.time = h->d_ev_i64.p;
+  ev.code = h->d_ev_u32.p;
+  TRY(dep_fire(h, ev, n, h->n_ent));
+  CU(cudaStreamSynchronize(h->stream));
   return CRANE_OK;
 }
 
@@ -1302,6 +1521,23 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
   }
   CU(cudaEventRecord(h->ev[kEvInitEnd], st));
 
+  // ---- the gate: held, not-yet-begun and dependent rows sit this run out ----
+  const bool gated = h->gate_on && N;
+  if (gated) {
+    TRY(gate_fit(h));
+    CU(h->d_g_code.ensure(N));
+    CRANE_LAUNCH(k_gate, (N + 255) / 256, 256, 0, st, gate_dev(h), now, h->d_g_code.p);
+    pd.dead = h->d_g_code.p;
+    h->timing.kernel_launches++;
+    // an account with only gated rows does not seed the fair-share bounds
+    if (h->n_accounts) {
+      CU(cudaMemsetAsync(h->d_acc_present.p, 0, h->n_accounts, st));
+      CRANE_LAUNCH(k_acc_present, (N + R + 255) / 256, 256, 0, st, h->d_account.p, h->d_g_code.p, N,
+                   h->d_rn_account.p, R, h->d_acc_present.p);
+      h->timing.kernel_launches++;
+    }
+  }
+
   // ---- priority + queue (R5,R6) --------------------------------------------
   uint32_t nq_cap = std::min<uint32_t>(N, h->cfg.scheduled_batch_size);
   CU(cudaMemsetAsync(h->d_part_count.p, 0, sizeof(uint32_t) * (h->n_vparts + 2), st));
@@ -1332,7 +1568,7 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     CRANE_LAUNCH(k_priority, (N + 255) / 256, 256, 0, st, pd, pc, now, h->d_bounds.p, h->d_acc_service.p,
                  h->d_prio.p, h->d_keys_a.p, h->d_vals_a.p);
     h->timing.kernel_launches++;
-    if (pc.type != 0 || h->n_dead)  // (FIFO keeps input order; erased rows only have to go behind the live ones)
+    if (pc.type != 0 || h->n_dead || gated)  // (FIFO keeps input order; excluded rows only have to go behind the others)
       TRY(radix_sort(h, N, pc.type != 0 ? 64 : 8, &keys, &vals));
     // keys2 go to the buffer not holding `vals`
     uint64_t* key2 = h->d_keys_a.p;

@@ -60,7 +60,8 @@ struct PendingDev {  // SoA mirror of crane_pending_t
   const uint32_t* excl_nodes;
   const uint32_t* alloc_off;  // exclusive prefix sum of node_num
   const uint32_t* reservation;  // or null
-  const uint8_t* dead;          // erased rows of the device-resident table (or null): not in the queue
+  const uint8_t* dead;          // erased rows of the device-resident table (or null): not in the queue; in a
+                                // gated run the row's exclusion code (ERASED or a gate reason)
 };
 
 struct RunningDev {
@@ -504,8 +505,8 @@ __global__ void k_queue_keys(PendingDev pd, const uint32_t* order, const double*
     p = cl.part_comp[p];
   }
   uint64_t k = 0;
-  if (pd.dead && pd.dead[j]) {
-    reason = CRANE_REASON_ERASED;
+  if (pd.dead && pd.dead[j]) {  // a tombstone (1) or the gate's code of the row (gate_kernels.cuh)
+    reason = pd.dead[j] == 1 ? (uint8_t)CRANE_REASON_ERASED : pd.dead[j];
     found = false;
     k = (uint64_t)cl.n_vparts + 1;
   } else if (r >= limit) {

@@ -83,6 +83,14 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.crane_sched_keep_running.argtypes = [C.c_void_p, P(C.c_float)]
     lib.crane_sched_running_rows.restype = C.c_uint32
     lib.crane_sched_running_rows.argtypes = [C.c_void_p]
+    lib.crane_sched_pending_set_gate.restype = C.c_int
+    lib.crane_sched_pending_set_gate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+    lib.crane_sched_pending_depend.restype = C.c_int
+    lib.crane_sched_pending_depend.argtypes = [C.c_void_p, P(abi.DependenciesC)]
+    lib.crane_sched_pending_cancel.restype = C.c_int
+    lib.crane_sched_pending_cancel.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int64]
+    lib.crane_sched_running_end.restype = C.c_int
+    lib.crane_sched_running_end.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     lib.crane_sched_set_shard.restype = C.c_int
     lib.crane_sched_set_shard.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
     lib.crane_sched_device_placements.restype = C.c_int
@@ -104,7 +112,9 @@ EXPORTS = ("crane_sched_create", "crane_sched_destroy", "crane_sched_last_error"
            "crane_sched_running_erase", "crane_sched_start", "crane_sched_keep_running", "crane_sched_running_rows",
            "crane_sched_run", "crane_sched_fetch", "crane_sched_sync", "crane_sched_get_timing",
            "crane_sched_qos_filter", "crane_sched_set_shard", "crane_sched_device_placements",
-           "crane_sched_debug_bitmap", "crane_sched_debug_profile", "crane_sched_schedule_steps")
+           "crane_sched_debug_bitmap", "crane_sched_debug_profile", "crane_sched_schedule_steps",
+           "crane_sched_pending_set_gate", "crane_sched_pending_depend", "crane_sched_pending_cancel",
+           "crane_sched_running_end")
 
 
 class GpuScheduler:
@@ -210,6 +220,38 @@ class GpuScheduler:
 
     def running_rows(self) -> int:
         return int(self._lib.crane_sched_running_rows(self._h))
+
+    # --- the gate of the resident pending table: hold, begin time, dependencies --------
+    def pending_set_gate(self, rows, held=None, begin_time=None):
+        """Hold flag and / or begin time of resident rows (None = unchanged)."""
+        r = np.ascontiguousarray(rows, np.uint32)
+        hd = None if held is None else np.ascontiguousarray(held, np.uint8)
+        bt = None if begin_time is None else np.ascontiguousarray(begin_time, np.int64)
+        for a in (hd, bt):
+            if a is not None and len(a) != len(r):
+                raise ValueError("pending_set_gate: one value per row")
+        self._check(self._lib.crane_sched_pending_set_gate(self._h, r.ctypes.data, len(r),
+                                                           None if hd is None else hd.ctypes.data,
+                                                           None if bt is None else bt.ctypes.data))
+
+    def pending_depend(self, deps: abi.Dependencies):
+        """Dependency lists of pending rows (SetDependency + AddDependent at submit)."""
+        c = deps.as_c()
+        self._check(self._lib.crane_sched_pending_depend(self._h, C.byref(c)))
+
+    def pending_cancel(self, rows, cancel_time: int):
+        """pending_erase of cancelled jobs plus their dependency events."""
+        r = np.ascontiguousarray(rows, np.uint32)
+        self._check(self._lib.crane_sched_pending_cancel(self._h, r.ctypes.data, len(r), cancel_time))
+
+    def running_end(self, rows, end_time, exit_code):
+        """running_erase of ended jobs plus their dependency events."""
+        r = np.ascontiguousarray(rows, np.uint32)
+        t = np.ascontiguousarray(end_time, np.int64)
+        c = np.ascontiguousarray(exit_code, np.uint32)
+        if len(t) != len(r) or len(c) != len(r):
+            raise ValueError("running_end: one end time and one exit code per row")
+        self._check(self._lib.crane_sched_running_end(self._h, r.ctypes.data, len(r), t.ctypes.data, c.ctypes.data))
 
     def run(self, now: int):
         self._check(self._lib.crane_sched_run(self._h, now))

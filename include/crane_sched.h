@@ -190,6 +190,11 @@ enum {
   CRANE_REASON_PART_NOT_FOUND = 4, /* "Partition Not Found"                   */
   CRANE_REASON_RESV_NOT_FOUND = 5, /* "Reservation Not Found" (JS.cpp:5793)   */
   CRANE_REASON_PREEMPTED = 6,      /* "Preempted" (JS.cpp:5815)               */
+  /* written for rows the gate keeps out of the run (JobScheduler.cpp:1090-1113) */
+  CRANE_REASON_HELD = 7,             /* "Held"                                */
+  CRANE_REASON_BEGIN_TIME = 8,       /* "BeginTime"                           */
+  CRANE_REASON_DEPENDENCY = 9,       /* "Dependency"                          */
+  CRANE_REASON_DEPENDENCY_NEVER = 10,/* "DependencyNeverSatisfied"            */
   /* written by crane_sched_qos_filter (Accounting/AccountMetaContainer.cpp:382-531) */
   CRANE_REASON_QOS_CPU = 16,       /* "QosCpuResourceLimit"                   */
   CRANE_REASON_QOS_JOBS = 17,      /* "QosJobsResourceLimit"                  */
@@ -327,6 +332,93 @@ int crane_sched_running_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n
 int crane_sched_start(crane_sched_t* h, const uint32_t* pending_rows, uint32_t n, uint32_t* first_row);
 int crane_sched_keep_running(crane_sched_t* h, float* device_ms);
 uint32_t crane_sched_running_rows(const crane_sched_t* h);
+
+/* ---- the gate of the resident pending table ----------------------------------- */
+/* Before NodeSelect the daemon leaves out of the pending vector every job that is held,
+ * whose begin time is still ahead, or whose dependencies are not met
+ * (JobScheduler.cpp:1090-1113). Such rows stay in the resident table: each run
+ * (crane_sched_run) first evaluates, per row and in this order,
+ *     held                                    -> CRANE_REASON_HELD
+ *     begin_time > now                        -> CRANE_REASON_BEGIN_TIME
+ *     dependencies not met (is_met(now))      -> CRANE_REASON_DEPENDENCY_NEVER if they
+ *                                                can never be met (is_failed), else
+ *                                                CRANE_REASON_DEPENDENCY
+ * and a gated row takes part in nothing, exactly as an erased row: not in the priority
+ * bounds, the fair-share account set, the batch limit or the queue. It reports its
+ * reason, start / end time 0, n_alloc 0 and zero allocation rows; its priority is
+ * unspecified (the daemon does not write it). The dependency state of a row is
+ * DependenciesInJob (CtldPublicDefs.h:413-428): entries not yet resolved, is_or and
+ * ready_time; an event of a dependee sets ready_time = is_or ? min(ready_time, t + delay)
+ * : max(ready_time, t + delay) and resolves the entry;
+ *     is_met(now) = (is_or || no entry left) && ready_time <= now
+ *     is_failed   = ready_time == CRANE_TIME_FUTURE && (!is_or || no entry left).
+ * Times: CRANE_TIME_PAST / CRANE_TIME_FUTURE stand for absl::InfinitePast / InfiniteFuture;
+ * t + delay saturates as absl does (an infinite t stays infinite, a finite sum beyond the
+ * int64 range is CRANE_TIME_FUTURE). Event times (cancel, end, begin) are whole seconds:
+ * the daemon's own carry sub-second parts while its `now` is truncated (JobScheduler.cpp:
+ * 1071), so round them UP to the next second. That keeps is_met / is_failed exactly as the
+ * daemon computes them, because min, max and + whole-second delays commute with ceil;
+ * truncating could let a dependent pass one tick early. A table on which no gate call was
+ * made since crane_sched_pending_reset (which clears all gate state) runs exactly as
+ * before. On a sharded handle every rank must issue the same gate calls, as it does
+ * uploads. Every call here needs set_cluster and voids the last run, like pending_erase. */
+#define CRANE_TIME_PAST INT64_MIN
+#define CRANE_TIME_FUTURE INT64_MAX
+
+/* DependencyType (PublicDefs.proto:136-141) */
+enum { CRANE_DEP_AFTER = 0, CRANE_DEP_AFTER_ANY = 1, CRANE_DEP_AFTER_OK = 2, CRANE_DEP_AFTER_NOT_OK = 3 };
+/* What a dependency entry waits on */
+enum {
+  CRANE_DEPENDEE_PENDING = 0, /* a pending row of this table                            */
+  CRANE_DEPENDEE_RUNNING = 1, /* a running row: AFTER resolves at once at its start time */
+  CRANE_DEPENDEE_EVENT = 2,   /* already resolved at event_time (recovery from the DB,
+                                 re-sending a row's state after compaction: one EVENT
+                                 entry at the row's ready_time reproduces it)           */
+};
+
+/* The dependency lists of pending rows (JobInCtld::SetDependency and AddDependent at
+ * submit, CtldPublicDefs.cpp:1600-1626; JobScheduler.cpp:4215-4248). Row k of the call is
+ * pending row row[k]; its entries are [dep_off[k], dep_off[k+1]). */
+typedef struct crane_dependencies {
+  uint32_t n;
+  const uint32_t* row;        /* [n] pending rows                                    */
+  const uint8_t* is_or;       /* [n] Dependencies::is_or                            */
+  const uint32_t* dep_off;    /* [n+1] CSR over the entries                          */
+  const uint8_t* kind;        /* CRANE_DEPENDEE_*                                    */
+  const uint32_t* dependee;   /* pending or running row (ignored for EVENT)          */
+  const uint8_t* type;        /* CRANE_DEP_*                                         */
+  const uint64_t* delay_s;    /* < 2^62                                              */
+  const int64_t* event_time;  /* EVENT entries; NULL when the call has none          */
+} crane_dependencies_t;
+
+/* set_gate: hold flag and begin time of resident rows (SetHeld, HoldReleaseJobAsync, a
+ *   begin-time change, submit); `held` or `begin_time` NULL = unchanged. A row that never
+ *   had one is not held and begins at CRANE_TIME_PAST.
+ * pending_depend: gives rows their dependency list. CRANE_EINVAL when a row is out of
+ *   range, erased, listed twice or already has a list, when a dependee row is out of
+ *   range, erased or ended (the daemon's missing-dependency rejection) or is the row
+ *   itself, when one row lists the same dependee twice, or for a type > 3, a kind > 2 or
+ *   a delay >= 2^62. A RUNNING dependee resolves an AFTER entry at once at its start time.
+ * pending_cancel: pending_erase of cancelled jobs, and their events (JobScheduler.cpp:
+ *   4067-4073): AFTER and AFTER_ANY at cancel_time, AFTER_OK and AFTER_NOT_OK at
+ *   CRANE_TIME_FUTURE.
+ * running_end: running_erase of ended jobs, and their events (JobScheduler.cpp:4531-4538)
+ *   at end_time[k] (the daemon's recorded end time): AFTER_ANY; AFTER_OK if exit_code[k]
+ *   == 0, else at CRANE_TIME_FUTURE; AFTER_NOT_OK the other way round.
+ * crane_sched_start also resolves the AFTER entries on the started rows at their
+ *   placement's start time (JobScheduler.cpp:1549); their other entries follow the job to
+ *   its new running row.
+ * pending_erase and running_erase fire nothing: a row with dependents leaves through
+ * pending_cancel or running_end. crane_sched_set_running replaces the running table, so
+ * entries waiting on running rows must be re-sent (pending_reset, pending_append,
+ * set_gate, pending_depend with EVENT entries for what was resolved) when it is used to
+ * compact a table with dependencies. */
+int crane_sched_pending_set_gate(crane_sched_t* h, const uint32_t* rows, uint32_t n, const uint8_t* held,
+                                 const int64_t* begin_time);
+int crane_sched_pending_depend(crane_sched_t* h, const crane_dependencies_t* deps);
+int crane_sched_pending_cancel(crane_sched_t* h, const uint32_t* rows, uint32_t n, int64_t cancel_time);
+int crane_sched_running_end(crane_sched_t* h, const uint32_t* rows, uint32_t n, const int64_t* end_time,
+                            const uint32_t* exit_code);
 
 /* Blocks until the handle's stream is idle; *run_ms (optional) receives the
  * device time of the last crane_sched_run (CUDA events on that stream). */
