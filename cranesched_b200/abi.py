@@ -866,3 +866,76 @@ class StepPlacements:
         for f in self.__dataclass_fields__:
             h.update(np.ascontiguousarray(getattr(self, f)).tobytes())
         return h.hexdigest()
+
+
+# ---------------------------------------------------------------------------
+# The step state of running jobs kept resident on the device (crane_sched_steps_run)
+# ---------------------------------------------------------------------------
+class StepResultsC(C.Structure):
+    """crane_step_results_t"""
+    _fields_ = [("step_row", _p), ("node_off", _p), ("alloc_node", _p), ("alloc_ntasks", _p), ("alloc_res", _p),
+                ("task_off", _p), ("task_node", _p), ("task_res", _p)]
+
+
+@dataclass
+class StepResults:
+    """What one resident pass scheduled: the step rows (ascending), their node rows
+    (node-index order) and task rows (task-id order), offsets over the returned steps."""
+    step_row: np.ndarray
+    node_off: np.ndarray
+    alloc_node: np.ndarray
+    alloc_ntasks: np.ndarray
+    alloc_res: np.ndarray
+    task_off: np.ndarray
+    task_node: np.ndarray
+    task_res: np.ndarray
+
+    @staticmethod
+    def sized(n_scheduled: int, n_node_rows: int, n_task_rows: int) -> "StepResults":
+        z = np.zeros
+        return StepResults(z(n_scheduled, np.uint32), z(n_scheduled + 1, np.uint32), z(n_node_rows, np.uint32),
+                           z(n_node_rows, np.uint32), z(n_node_rows, RES_IN_NODE), z(n_scheduled + 1, np.uint32),
+                           z(n_task_rows, np.uint32), z(n_task_rows, RES_IN_NODE))
+
+    @property
+    def n(self):
+        return len(self.step_row)
+
+    def as_c(self) -> StepResultsC:
+        return StepResultsC(*[_ptr(getattr(self, f)) for f in self.__dataclass_fields__])
+
+    def diff(self, other: "StepResults") -> list[str]:
+        return StepPlacements.diff(self, other)
+
+    def digest(self) -> str:
+        return StepPlacements.digest(self)
+
+    def expand(self, step_rows, job_step_off, steps: Steps) -> StepPlacements:
+        """The StepPlacements crane_sched_schedule_steps writes for `steps`, whose row s
+        is resident step row step_rows[s] and whose jobs own the rows
+        [job_step_off[j], job_step_off[j+1]): steps outside the results are not scheduled
+        (their rows zero), `placed` counts a job's scheduled steps."""
+        step_rows = np.asarray(step_rows, np.int64)
+        job_step_off = np.asarray(job_step_off, np.int64)
+        out = StepPlacements.for_steps(StepJobs(np.zeros(len(job_step_off), np.uint32), np.zeros(0, np.uint32),
+                                                np.zeros(0, RES_IN_NODE), job_step_off), steps)
+        out.node_off[1:] = np.cumsum(steps.node_num, dtype=np.int64)
+        out.task_off[1:] = np.cumsum(steps.ntasks, dtype=np.int64)
+        at = np.searchsorted(self.step_row, step_rows)
+        hit = (at < self.n) & (self.step_row[np.minimum(at, max(self.n - 1, 0))] == step_rows) if self.n else \
+            np.zeros(len(step_rows), bool)
+        if int(hit.sum()) != self.n:
+            raise ValueError("StepResults.expand: a returned step is not in the given step set")
+        out.scheduled[hit] = 1
+        for s in np.flatnonzero(hit):
+            r = at[s]
+            d0, n0, n1 = out.node_off[s], self.node_off[r], self.node_off[r + 1]
+            out.alloc_node[d0:d0 + n1 - n0] = self.alloc_node[n0:n1]
+            out.alloc_ntasks[d0:d0 + n1 - n0] = self.alloc_ntasks[n0:n1]
+            out.alloc_res[d0:d0 + n1 - n0] = self.alloc_res[n0:n1]
+            d0, t0, t1 = out.task_off[s], self.task_off[r], self.task_off[r + 1]
+            out.task_node[d0:d0 + t1 - t0] = self.task_node[t0:t1]
+            out.task_res[d0:d0 + t1 - t0] = self.task_res[t0:t1]
+        job = np.repeat(np.arange(len(job_step_off) - 1), np.diff(job_step_off))
+        np.add.at(out.placed, job[hit], 1)
+        return out

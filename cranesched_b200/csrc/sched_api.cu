@@ -32,6 +32,7 @@
 #include "step_kernels.cuh"
 #include "running_kernels.cuh"
 #include "gate_kernels.cuh"
+#include "step_resident_kernels.cuh"
 
 using namespace crane;
 
@@ -88,6 +89,7 @@ enum Ev {
   kEvQosBegin, kEvQosEnd,                                                  // qos_filter
   kEvStepsBegin, kEvStepsEnd,                                              // schedule_steps
   kEvKeepBegin, kEvKeepEnd,                                                // keep_running
+  kEvSpBegin, kEvSpMid, kEvSpScatter, kEvSpEnd,                            // steps_run
   kNumEv
 };
 
@@ -226,6 +228,30 @@ struct crane_sched {
   DBuf<Row> d_st_rows;       // avail | alloc_res | task_res
   DBuf<View> d_st_views;     // req_node | req_task
   DBuf<uint8_t> d_st_sched;
+  // resident step state (step_resident_kernels.cuh): host mirrors of the small columns
+  uint32_t n_sj = 0, n_sp = 0, n_sa = 0;        // step-job rows, step rows, allocation-pool rows
+  std::vector<uint32_t> h_sj_node_off = {0};    // [n_sj + 1]
+  std::vector<uint8_t> h_sj_dead, h_sj_dirty;
+  std::vector<std::vector<uint32_t>> h_sj_queue;  // live pending step rows of each job, row order
+  std::vector<uint32_t> h_sj_dirty_rows;        // the rows with h_sj_dirty set
+  std::vector<uint32_t> h_sp_job, h_sp_nn, h_sp_nt, h_sp_incl_off = {0}, h_sp_excl_off = {0};
+  std::vector<uint8_t> h_sp_state;              // kSpPending, kSpScheduled, kSpErased
+  DBuf<uint32_t> d_sj_node_off, d_sj_node;
+  DBuf<Row> d_sj_avail;
+  DBuf<uint32_t> d_sp_job, d_sp_nn, d_sp_nt, d_sp_t0, d_sp_t1, d_sp_incl_off, d_sp_incl, d_sp_excl_off, d_sp_excl,
+      d_sp_alloc_at;
+  DBuf<View> d_sp_req_node, d_sp_req_task;
+  DBuf<uint32_t> d_sa_node;
+  DBuf<Row> d_sa_res;
+  // the last pass: the dense tables, its results and what the host knows of them
+  DBuf<uint32_t> d_sq_u32, d_sr_u32;            // dense u32 columns | results: ntasks, task_node
+  DBuf<Row> d_sq_rows, d_sr_rows;               // dense avail, alloc_res, task_res | results: task_res
+  DBuf<View> d_sq_views;
+  DBuf<uint8_t> d_sq_sched;
+  DBuf<uint32_t> d_sp_call, d_sp_flag;          // per call: rows and offsets | the seed's check
+  bool sp_results = false;                      // steps_fetch may be called
+  uint32_t sr_sa_base = 0;
+  std::vector<uint32_t> h_sr_rows, h_sr_node_off, h_sr_task_off;
 
   // the buffers free themselves after this, on the handle's device
   ~crane_sched() {
@@ -290,6 +316,32 @@ int check_node_list(crane_sched* h, const char* what, const uint32_t* off, const
   if (off[n] && !nodes) return fail(h, CRANE_EINVAL, "%s: node list CSR without node array", what);
   for (uint32_t k = 0; k < off[n]; ++k)
     if (nodes[k] >= h->n_nodes && nodes[k] != 0xFFFFFFFFu) return fail(h, CRANE_EINVAL, "%s: listed node out of range", what);
+  return CRANE_OK;
+}
+
+// The rows of a crane_steps_t (crane_sched_schedule_steps, crane_sched_steps_append);
+// *nrows / *trows = their node / task rows
+int check_steps(crane_sched* h, const crane_steps_t* st, uint64_t* nrows, uint64_t* trows) {
+  const uint32_t S = st->n;
+  if (S && (!st->node_num || !st->ntasks || !st->ntasks_per_node_min || !st->ntasks_per_node_max || !st->req_node ||
+            !st->req_task))
+    return fail(h, CRANE_EINVAL, "steps: null column");
+  *nrows = *trows = 0;
+  for (uint32_t s = 0; s < S; ++s) {
+    const uint32_t nn = st->node_num[s], nt = st->ntasks[s], t0 = st->ntasks_per_node_min[s], t1 = st->ntasks_per_node_max[s];
+    if (nn == 0) return fail(h, CRANE_EINVAL, "steps[%u]: node_num == 0", s);
+    if (nt < nn) return fail(h, CRANE_EINVAL, "steps[%u]: ntasks < node_num", s);
+    if (t0 > t1) return fail(h, CRANE_EINVAL, "steps[%u]: ntasks_per_node_min > ntasks_per_node_max", s);
+    if (nn >= (uint32_t)kStepHeapMax) return fail(h, CRANE_ENOSYS, "steps[%u]: node_num above %d", s, kStepHeapMax - 1);
+    // (a node could then be picked for no task; the reference hands it ntasks - node_num + 1 unchecked allocations)
+    if (t0 == 0) return fail(h, CRANE_ENOSYS, "steps[%u]: ntasks_per_node_min == 0", s);
+    if (st->req_node[s].cpu_raw < 0 || st->req_task[s].cpu_raw < 0) return fail(h, CRANE_EINVAL, "steps[%u]: negative cpu request", s);
+    *nrows += nn;
+    *trows += nt;
+  }
+  if (*nrows > 0xfffffff0ull || *trows > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "steps: too many node / task rows");
+  if (st->incl_off) TRY(check_node_list(h, "steps: include list", st->incl_off, st->incl_nodes, S));
+  if (st->excl_off) TRY(check_node_list(h, "steps: exclude list", st->excl_off, st->excl_nodes, S));
   return CRANE_OK;
 }
 
@@ -1814,25 +1866,8 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
       if (k > jb->node_off[j] && jb->node[k] <= jb->node[k - 1])
         return fail(h, CRANE_EINVAL, "step jobs[%u]: nodes must be ascending and distinct", j);
     }
-  if (S && (!st->node_num || !st->ntasks || !st->ntasks_per_node_min || !st->ntasks_per_node_max || !st->req_node ||
-            !st->req_task))
-    return fail(h, CRANE_EINVAL, "steps: null column");
   uint64_t nrows = 0, trows = 0;
-  for (uint32_t s = 0; s < S; ++s) {
-    const uint32_t nn = st->node_num[s], nt = st->ntasks[s], t0 = st->ntasks_per_node_min[s], t1 = st->ntasks_per_node_max[s];
-    if (nn == 0) return fail(h, CRANE_EINVAL, "steps[%u]: node_num == 0", s);
-    if (nt < nn) return fail(h, CRANE_EINVAL, "steps[%u]: ntasks < node_num", s);
-    if (t0 > t1) return fail(h, CRANE_EINVAL, "steps[%u]: ntasks_per_node_min > ntasks_per_node_max", s);
-    if (nn >= (uint32_t)kStepHeapMax) return fail(h, CRANE_ENOSYS, "steps[%u]: node_num above %d", s, kStepHeapMax - 1);
-    // (a node could then be picked for no task; the reference hands it ntasks - node_num + 1 unchecked allocations)
-    if (t0 == 0) return fail(h, CRANE_ENOSYS, "steps[%u]: ntasks_per_node_min == 0", s);
-    if (st->req_node[s].cpu_raw < 0 || st->req_task[s].cpu_raw < 0) return fail(h, CRANE_EINVAL, "steps[%u]: negative cpu request", s);
-    nrows += nn;
-    trows += nt;
-  }
-  if (nrows > 0xfffffff0ull || trows > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "steps: too many node / task rows");
-  if (st->incl_off) TRY(check_node_list(h, "steps: include list", st->incl_off, st->incl_nodes, S));
-  if (st->excl_off) TRY(check_node_list(h, "steps: exclude list", st->excl_off, st->excl_nodes, S));
+  TRY(check_steps(h, st, &nrows, &trows));
   if ((J && !out->placed) || (S && (!out->scheduled || !out->node_off || !out->task_off)) || !out->node_off || !out->task_off ||
       (nrows && (!out->alloc_node || !out->alloc_ntasks || !out->alloc_res)) || (trows && (!out->task_node || !out->task_res)))
     return fail(h, CRANE_EINVAL, "step placements: null column");
@@ -1905,6 +1940,462 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
   CU(cudaStreamSynchronize(sm));
   CU(cudaGetLastError());
   if (device_ms) *device_ms = elapsed_ms(h, kEvStepsBegin, kEvStepsEnd);
+  return CRANE_OK;
+}
+
+}  // extern "C"
+
+// ---- the step state of running jobs, resident on the device -------------------------
+namespace {
+
+enum : uint8_t { kSpPending = 0, kSpScheduled = 1, kSpErased = 2 };
+
+void sj_dirty(crane_sched* h, uint32_t j) {
+  if (!h->h_sj_dirty[j]) {
+    h->h_sj_dirty[j] = 1;
+    h->h_sj_dirty_rows.push_back(j);
+  }
+}
+
+// The rows of an erase / start / read call: in [0, n_rows), not erased, none listed twice
+template <class Erased>
+int check_rows(crane_sched* h, const char* call, const uint32_t* rows, uint32_t n, uint32_t n_rows, Erased erased) {
+  if (n && !rows) return fail(h, CRANE_EINVAL, "%s: null rows", call);
+  std::vector<uint32_t> sorted(rows, rows + n);
+  std::sort(sorted.begin(), sorted.end());
+  for (uint32_t k = 0; k < n; ++k) {
+    if (sorted[k] >= n_rows) return fail(h, CRANE_EINVAL, "%s: row %u out of range", call, sorted[k]);
+    if (erased(sorted[k])) return fail(h, CRANE_EINVAL, "%s: row %u was erased", call, sorted[k]);
+    if (k && sorted[k] == sorted[k - 1]) return fail(h, CRANE_EINVAL, "%s: row %u listed twice", call, sorted[k]);
+  }
+  return CRANE_OK;
+}
+
+// New step-job rows whose nodes and avail are in the pools up to off.back()
+void sj_commit(crane_sched* h, const std::vector<uint32_t>& off) {
+  for (size_t k = 0; k + 1 < off.size(); ++k) {
+    h->h_sj_node_off.push_back(off[k + 1]);
+    h->h_sj_dead.push_back(0);
+    h->h_sj_dirty.push_back(0);
+    h->h_sj_queue.emplace_back();
+    sj_dirty(h, h->n_sj++);
+  }
+}
+
+StepPoolDev step_pool(crane_sched* h) {
+  StepPoolDev p{};
+  p.sj_node_off = h->d_sj_node_off.p;
+  p.sj_node = h->d_sj_node.p;
+  p.sj_avail = h->d_sj_avail.p;
+  p.job = h->d_sp_job.p;
+  p.node_num = h->d_sp_nn.p;
+  p.ntasks = h->d_sp_nt.p;
+  p.ntpn_min = h->d_sp_t0.p;
+  p.ntpn_max = h->d_sp_t1.p;
+  p.req_node = h->d_sp_req_node.p;
+  p.req_task = h->d_sp_req_task.p;
+  p.incl_off = h->d_sp_incl_off.p;
+  p.incl_nodes = h->d_sp_incl.p;
+  p.excl_off = h->d_sp_excl_off.p;
+  p.excl_nodes = h->d_sp_excl.p;
+  p.alloc_at = h->d_sp_alloc_at.p;
+  p.sa_node = h->d_sa_node.p;
+  p.sa_res = h->d_sa_res.p;
+  return p;
+}
+
+// grid of a kernel with one warp per item, 256 threads per block
+uint32_t warp_grid(const crane_sched* h, uint64_t items) {
+  return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((items + 7) / 8, 8ull * h->n_sm));
+}
+
+}  // namespace
+
+extern "C" {
+
+int crane_sched_step_jobs_reset(crane_sched_t* h) {
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "step_jobs_reset"));
+  h->n_sj = h->n_sp = h->n_sa = 0;
+  h->h_sj_node_off.assign(1, 0);
+  h->h_sj_dead.clear();
+  h->h_sj_dirty.clear();
+  h->h_sj_queue.clear();
+  h->h_sj_dirty_rows.clear();
+  h->h_sp_job.clear();
+  h->h_sp_nn.clear();
+  h->h_sp_nt.clear();
+  h->h_sp_state.clear();
+  h->h_sp_incl_off.assign(1, 0);
+  h->h_sp_excl_off.assign(1, 0);
+  h->sp_results = false;
+  return CRANE_OK;
+}
+
+int crane_sched_step_jobs_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32_t* first) {
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "step_jobs_start"));
+  TRY(check_rows(h, "step_jobs_start", rows, n, h->n_rr, [&](uint32_t r) { return h->h_rr_dead[r] != 0; }));
+  CU(cudaSetDevice(h->device));
+  h->sp_results = false;
+  cudaStream_t st = h->stream;
+  const uint32_t base = h->n_sj, eb = h->h_sj_node_off.back();
+  std::vector<uint32_t> off(n + 1, eb);
+  for (uint32_t k = 0; k < n; ++k) {
+    const uint64_t e = (uint64_t)off[k] + (h->h_rr_alloc_off[rows[k] + 1] - h->h_rr_alloc_off[rows[k]]);
+    if (e > 0xfffffff0ull || (uint64_t)base + n > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "step_jobs_start: too many rows");
+    off[k + 1] = (uint32_t)e;
+  }
+  if (n) {
+    CU(h->d_sj_node.grow(off[n], eb, st));
+    CU(h->d_sj_avail.grow(off[n], eb, st));
+    H2D_AT(h->d_sj_node_off, off.data(), base, (size_t)n + 1);
+    H2D(h->d_sp_call, rows, n);
+    CU(h->d_sp_flag.ensure(1));
+    CU(cudaMemsetAsync(h->d_sp_flag.p, 0, sizeof(uint32_t), st));
+    CRANE_LAUNCH(k_sj_seed, warp_grid(h, n), 256, 0, st, h->d_rr_alloc_off.p, h->d_rr_alloc_node.p, h->d_rr_alloc_res.p,
+                 h->d_sp_call.p, n, h->d_sj_node_off.p + base, h->d_sj_node.p, h->d_sj_avail.p, h->d_sp_flag.p);
+    uint32_t bad = 0;
+    CU(cudaMemcpyAsync(&bad, h->d_sp_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    if (bad) return fail(h, CRANE_EINVAL, "step_jobs_start: a running row's allocation nodes are not ascending and distinct");
+  }
+  sj_commit(h, off);
+  if (first) *first = base;
+  return CRANE_OK;
+}
+
+int crane_sched_step_jobs_append(crane_sched_t* h, const crane_step_jobs_t* jb, uint32_t* first) {
+  if (!h || !jb) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "step_jobs_append"));
+  if (jb->step_off) return fail(h, CRANE_EINVAL, "step_jobs_append: step_off must be NULL (steps come with steps_append)");
+  const uint32_t J = jb->n_jobs;
+  TRY(check_offsets(h, "step jobs: node_off", jb->node_off, J));
+  const uint32_t E = jb->node_off[J];
+  if (E && (!jb->node || !jb->avail)) return fail(h, CRANE_EINVAL, "step jobs: null node table");
+  for (uint32_t j = 0; j < J; ++j)
+    for (uint32_t k = jb->node_off[j]; k < jb->node_off[j + 1]; ++k) {
+      if (jb->node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "step jobs[%u]: node %u out of range", j, jb->node[k]);
+      if (k > jb->node_off[j] && jb->node[k] <= jb->node[k - 1])
+        return fail(h, CRANE_EINVAL, "step jobs[%u]: nodes must be ascending and distinct", j);
+    }
+  const uint32_t base = h->n_sj, eb = h->h_sj_node_off.back();
+  if ((uint64_t)eb + E > 0xfffffff0ull || (uint64_t)base + J > 0xfffffff0ull)
+    return fail(h, CRANE_EINVAL, "step_jobs_append: too many rows");
+  CU(cudaSetDevice(h->device));
+  h->sp_results = false;
+  std::vector<uint32_t> off(J + 1);
+  for (uint32_t j = 0; j <= J; ++j) off[j] = eb + jb->node_off[j];
+  H2D_AT(h->d_sj_node_off, off.data(), base, (size_t)J + 1);
+  H2D_AT(h->d_sj_node, jb->node, eb, E);
+  H2D_AT(h->d_sj_avail, reinterpret_cast<const Row*>(jb->avail), eb, E);
+  CU(cudaStreamSynchronize(h->stream));  // (the staging vector is pageable)
+  sj_commit(h, off);
+  if (first) *first = base;
+  return CRANE_OK;
+}
+
+int crane_sched_step_jobs_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n) {
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "step_jobs_erase"));
+  TRY(check_rows(h, "step_jobs_erase", rows, n, h->n_sj, [&](uint32_t r) { return h->h_sj_dead[r] != 0; }));
+  h->sp_results = false;
+  for (uint32_t k = 0; k < n; ++k) {  // its step rows go with it: every check looks at the job
+    h->h_sj_dead[rows[k]] = 1;
+    std::vector<uint32_t>().swap(h->h_sj_queue[rows[k]]);
+  }
+  return CRANE_OK;
+}
+
+int crane_sched_steps_append(crane_sched_t* h, const crane_steps_t* st, const uint32_t* job_row, uint32_t* first) {
+  if (!h || !st) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "steps_append"));
+  const uint32_t S = st->n;
+  uint64_t nrows = 0, trows = 0;
+  TRY(check_steps(h, st, &nrows, &trows));
+  if (S && !job_row) return fail(h, CRANE_EINVAL, "steps_append: null job_row");
+  for (uint32_t s = 0; s < S; ++s) {
+    if (job_row[s] >= h->n_sj) return fail(h, CRANE_EINVAL, "steps_append[%u]: job row %u out of range", s, job_row[s]);
+    if (h->h_sj_dead[job_row[s]]) return fail(h, CRANE_EINVAL, "steps_append[%u]: job row %u was erased", s, job_row[s]);
+  }
+  const uint32_t base = h->n_sp, ib = h->h_sp_incl_off.back(), xb = h->h_sp_excl_off.back();
+  const uint32_t ni = st->incl_off ? st->incl_off[S] : 0, nx = st->excl_off ? st->excl_off[S] : 0;
+  if ((uint64_t)base + S > 0xfffffff0ull || (uint64_t)ib + ni > 0xfffffff0ull || (uint64_t)xb + nx > 0xfffffff0ull)
+    return fail(h, CRANE_EINVAL, "steps_append: too many rows");
+  CU(cudaSetDevice(h->device));
+  h->sp_results = false;
+  std::vector<uint32_t> io(S + 1), xo(S + 1);
+  for (uint32_t s = 0; s <= S; ++s) {
+    io[s] = ib + (st->incl_off ? st->incl_off[s] : 0);
+    xo[s] = xb + (st->excl_off ? st->excl_off[s] : 0);
+  }
+  H2D_AT(h->d_sp_job, job_row, base, S);
+  H2D_AT(h->d_sp_nn, st->node_num, base, S);
+  H2D_AT(h->d_sp_nt, st->ntasks, base, S);
+  H2D_AT(h->d_sp_t0, st->ntasks_per_node_min, base, S);
+  H2D_AT(h->d_sp_t1, st->ntasks_per_node_max, base, S);
+  H2D_AT(h->d_sp_req_node, reinterpret_cast<const View*>(st->req_node), base, S);
+  H2D_AT(h->d_sp_req_task, reinterpret_cast<const View*>(st->req_task), base, S);
+  H2D_AT(h->d_sp_incl_off, io.data(), base, (size_t)S + 1);
+  H2D_AT(h->d_sp_excl_off, xo.data(), base, (size_t)S + 1);
+  H2D_AT(h->d_sp_incl, st->incl_nodes, ib, ni);
+  H2D_AT(h->d_sp_excl, st->excl_nodes, xb, nx);
+  CU(h->d_sp_alloc_at.grow(std::max<size_t>((size_t)base + S, 1), base, h->stream));
+  CU(cudaStreamSynchronize(h->stream));  // (the staging vectors are pageable)
+  for (uint32_t s = 0; s < S; ++s) {
+    h->h_sp_job.push_back(job_row[s]);
+    h->h_sp_nn.push_back(st->node_num[s]);
+    h->h_sp_nt.push_back(st->ntasks[s]);
+    h->h_sp_state.push_back(kSpPending);
+    h->h_sp_incl_off.push_back(io[s + 1]);
+    h->h_sp_excl_off.push_back(xo[s + 1]);
+    h->h_sj_queue[job_row[s]].push_back(base + s);
+    sj_dirty(h, job_row[s]);
+  }
+  h->n_sp = base + S;
+  if (first) *first = base;
+  return CRANE_OK;
+}
+
+int crane_sched_steps_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n) {
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "steps_erase"));
+  TRY(check_rows(h, "steps_erase", rows, n, h->n_sp, [&](uint32_t r) {
+    return h->h_sp_state[r] == kSpErased || h->h_sj_dead[h->h_sp_job[r]];
+  }));
+  CU(cudaSetDevice(h->device));
+  h->sp_results = false;
+  // scheduled rows give their node rows back, job by job, in row order
+  std::vector<std::pair<uint32_t, uint32_t>> rel;  // (job, step row)
+  for (uint32_t k = 0; k < n; ++k) {
+    const uint32_t s = rows[k], j = h->h_sp_job[s];
+    if (h->h_sp_state[s] == kSpScheduled) {
+      rel.emplace_back(j, s);
+    } else {
+      auto& q = h->h_sj_queue[j];
+      q.erase(std::find(q.begin(), q.end(), s));
+    }
+    h->h_sp_state[s] = kSpErased;
+    sj_dirty(h, j);
+  }
+  if (rel.empty()) return CRANE_OK;
+  std::sort(rel.begin(), rel.end());
+  std::vector<uint32_t> jobs, off{0}, steps;  // uploaded as one table: jobs | off | steps
+  for (size_t q = 0; q < rel.size(); ++q) {
+    if (q == 0 || rel[q].first != rel[q - 1].first) {
+      if (q) off.push_back((uint32_t)q);
+      jobs.push_back(rel[q].first);
+    }
+    steps.push_back(rel[q].second);
+  }
+  off.push_back((uint32_t)rel.size());
+  const uint32_t m = (uint32_t)jobs.size();
+  std::vector<uint32_t> u(jobs);
+  u.insert(u.end(), off.begin(), off.end());
+  u.insert(u.end(), steps.begin(), steps.end());
+  H2D(h->d_sp_call, u.data(), u.size());
+  const uint32_t* du = h->d_sp_call.p;
+  CRANE_LAUNCH(k_sp_release, warp_grid(h, m), 256, 0, h->stream, step_pool(h), du, du + m, du + 2 * m + 1, m);
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(h->stream));
+  return CRANE_OK;
+}
+
+int crane_sched_steps_run(crane_sched_t* h, uint32_t* n_scheduled, uint32_t* n_node_rows, uint32_t* n_task_rows,
+                          float* device_ms) {
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "steps_run"));
+  CU(cudaSetDevice(h->device));
+  (void)cudaGetLastError();
+  cudaStream_t sm = h->stream;
+  h->sp_results = false;
+  // the pass visits the dirty jobs with a live pending step, ascending, each with its queue
+  std::sort(h->h_sj_dirty_rows.begin(), h->h_sj_dirty_rows.end());
+  std::vector<uint32_t> u;  // jl | sl
+  for (uint32_t j : h->h_sj_dirty_rows) {
+    h->h_sj_dirty[j] = 0;
+    if (!h->h_sj_dead[j] && !h->h_sj_queue[j].empty()) u.push_back(j);
+  }
+  h->h_sj_dirty_rows.clear();
+  const uint32_t J = (uint32_t)u.size();
+  uint64_t E = 0, Li = 0, Le = 0, N = 0, T = 0;
+  for (uint32_t w = 0; w < J; ++w) {
+    const uint32_t j = u[w];
+    E += h->h_sj_node_off[j + 1] - h->h_sj_node_off[j];
+    for (uint32_t s : h->h_sj_queue[j]) {
+      u.push_back(s);
+      Li += h->h_sp_incl_off[s + 1] - h->h_sp_incl_off[s];
+      Le += h->h_sp_excl_off[s + 1] - h->h_sp_excl_off[s];
+      N += h->h_sp_nn[s];
+      T += h->h_sp_nt[s];
+    }
+  }
+  const uint32_t S = (uint32_t)(u.size() - J);
+  if (N > 0xfffffff0ull || T > 0xfffffff0ull || (uint64_t)h->n_sa + N > 0xfffffff0ull)
+    return fail(h, CRANE_EINVAL, "steps_run: too many node / task rows");
+  h->h_sr_rows.clear();
+  h->h_sr_node_off.assign(1, 0);
+  h->h_sr_task_off.assign(1, 0);
+  h->sr_sa_base = h->n_sa;
+  float ms = 0.f;
+  if (J) {
+    // dense u32 columns: jl | sl | node_off | node | step_off | nn | nt | t0 | t1 | incl_off | incl | excl_off | excl |
+    //                    out node_off | out task_off | placed | alloc_node | alloc_ntasks | task_node | pos
+    size_t at = 0;
+    auto take = [&](uint64_t n) { const size_t a = at; at += n; return a; };
+    const size_t o_jl = take(J), o_sl = take(S), o_noff = take(J + 1), o_node = take(E), o_soff = take(J + 1);
+    const size_t o_nn = take(S), o_nt = take(S), o_t0 = take(S), o_t1 = take(S);
+    const size_t o_io = take(S + 1), o_in = take(Li), o_xo = take(S + 1), o_xn = take(Le);
+    const size_t o_ooff = take(S + 1), o_toff = take(S + 1), o_placed = take(J);
+    const size_t o_anode = take(N), o_antasks = take(N), o_tnode = take(T), o_pos = take(2 * (uint64_t)S);
+    CU(h->d_sq_u32.ensure(at));
+    CU(h->d_sq_rows.ensure(std::max<uint64_t>(E + N + T, 1)));
+    CU(h->d_sq_views.ensure(2 * (size_t)S));
+    CU(h->d_sq_sched.ensure(S));
+    uint32_t* du = h->d_sq_u32.p;
+    Row* dr = h->d_sq_rows.p;
+    StepPassDev d{};
+    d.n_jobs = J;
+    d.n_steps = S;
+    d.jl = du + o_jl;
+    d.sl = du + o_sl;
+    d.node_off = du + o_noff;
+    d.node = du + o_node;
+    d.avail = dr;
+    d.step_off = du + o_soff;
+    d.node_num = du + o_nn;
+    d.ntasks = du + o_nt;
+    d.ntpn_min = du + o_t0;
+    d.ntpn_max = du + o_t1;
+    d.req_node = h->d_sq_views.p;
+    d.req_task = h->d_sq_views.p + S;
+    d.incl_off = du + o_io;
+    d.incl_nodes = du + o_in;
+    d.excl_off = du + o_xo;
+    d.excl_nodes = du + o_xn;
+    d.out_node_off = du + o_ooff;
+    d.out_task_off = du + o_toff;
+    d.placed = du + o_placed;
+    d.scheduled = h->d_sq_sched.p;
+    d.alloc_node = du + o_anode;
+    d.alloc_ntasks = du + o_antasks;
+    d.task_node = du + o_tnode;
+    d.alloc_res = dr + E;
+    d.task_res = dr + E + N;
+    CU(cudaMemcpyAsync(du, u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, sm));
+    CU(cudaEventRecord(h->ev[kEvSpBegin], sm));
+    const uint32_t mx = std::max(J, S) + 1;
+    CRANE_LAUNCH(k_sp_pass_cols, std::min<uint32_t>((mx + 255) / 256, 8 * h->n_sm), 256, 0, sm, step_pool(h), d);
+    ScanSegs sg{{d.node_off, d.incl_off, d.excl_off, d.out_node_off, d.out_task_off}, {J + 1, S + 1, S + 1, S + 1, S + 1}};
+    CRANE_LAUNCH(k_sp_scan, 1, 1024, 0, sm, sg);
+    CRANE_LAUNCH(k_sp_pass_rows, warp_grid(h, (uint64_t)J + S), 256, 0, sm, step_pool(h), d);
+    StepJobsDev dj{J, d.node_off, d.node, d.avail, d.step_off};
+    StepsDev ds{d.node_num, d.ntasks, d.ntpn_min, d.ntpn_max, d.req_node, d.req_task,
+                d.incl_off, d.incl_nodes, d.excl_off, d.excl_nodes};
+    StepOutDev dout{d.placed, d.scheduled, d.out_node_off, d.alloc_node, d.alloc_ntasks, d.alloc_res,
+                    d.out_task_off, d.task_node, d.task_res};
+    const uint32_t grid = std::min<uint32_t>((J + kStepWarps - 1) / kStepWarps, 16 * h->n_sm);
+    CRANE_LAUNCH(k_steps, grid, 32 * kStepWarps, 0, sm, dj, ds, dout, (uint32_t)h->dict_slot);
+    CU(cudaEventRecord(h->ev[kEvSpMid], sm));
+    std::vector<uint8_t> sched(S);
+    CU(cudaMemcpyAsync(sched.data(), d.scheduled, S, cudaMemcpyDeviceToHost, sm));
+    CU(cudaStreamSynchronize(sm));
+    CU(cudaGetLastError());
+    // the results are the scheduled steps in ascending step-row order: their row positions
+    std::vector<std::pair<uint32_t, uint32_t>> got;  // (step row, pass index)
+    for (uint32_t i = 0; i < S; ++i)
+      if (sched[i]) got.emplace_back(u[J + i], i);
+    std::sort(got.begin(), got.end());
+    std::vector<uint32_t> pos(2 * (size_t)S, 0);
+    for (const auto& g : got) {
+      const uint32_t s = g.first;
+      pos[2 * (size_t)g.second] = h->h_sr_node_off.back();
+      pos[2 * (size_t)g.second + 1] = h->h_sr_task_off.back();
+      h->h_sr_rows.push_back(s);
+      h->h_sr_node_off.push_back(h->h_sr_node_off.back() + h->h_sp_nn[s]);
+      h->h_sr_task_off.push_back(h->h_sr_task_off.back() + h->h_sp_nt[s]);
+    }
+    const uint32_t Nr = h->h_sr_node_off.back(), Tr = h->h_sr_task_off.back();
+    if (!got.empty()) {
+      CU(h->d_sa_node.grow((size_t)h->n_sa + Nr, h->n_sa, sm));
+      CU(h->d_sa_res.grow((size_t)h->n_sa + Nr, h->n_sa, sm));
+      CU(h->d_sr_u32.ensure((size_t)Nr + Tr));
+      CU(h->d_sr_rows.ensure(std::max<uint32_t>(Tr, 1)));
+      CU(cudaMemcpyAsync(du + o_pos, pos.data(), pos.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, sm));
+      CU(cudaEventRecord(h->ev[kEvSpScatter], sm));
+      CRANE_LAUNCH(k_sp_scatter, warp_grid(h, (uint64_t)J + S), 256, 0, sm, step_pool(h), d, du + o_pos, h->n_sa,
+                   h->d_sr_u32.p, h->d_sr_u32.p + Nr, h->d_sr_rows.p);
+      CU(cudaEventRecord(h->ev[kEvSpEnd], sm));
+      CU(cudaStreamSynchronize(sm));
+      CU(cudaGetLastError());
+      ms = elapsed_ms(h, kEvSpScatter, kEvSpEnd);
+    }
+    ms += elapsed_ms(h, kEvSpBegin, kEvSpMid);
+    // mirrors: the scheduled steps are the head of their job's queue
+    uint32_t i = 0;
+    for (uint32_t w = 0; w < J; ++w) {
+      auto& q = h->h_sj_queue[u[w]];
+      size_t k = 0;
+      for (const size_t len = q.size(); k < len && sched[i + k]; ++k) h->h_sp_state[q[k]] = kSpScheduled;
+      i += (uint32_t)q.size();
+      q.erase(q.begin(), q.begin() + k);
+    }
+    h->n_sa += Nr;
+  }
+  if (n_scheduled) *n_scheduled = (uint32_t)h->h_sr_rows.size();
+  if (n_node_rows) *n_node_rows = h->h_sr_node_off.back();
+  if (n_task_rows) *n_task_rows = h->h_sr_task_off.back();
+  if (device_ms) *device_ms = ms;
+  h->sp_results = true;
+  return CRANE_OK;
+}
+
+int crane_sched_steps_fetch(crane_sched_t* h, crane_step_results_t* out) {
+  if (!h || !out) return CRANE_EINVAL;
+  if (!h->sp_results) return fail(h, CRANE_EINVAL, "steps_fetch: steps_run first");
+  const size_t Ns = h->h_sr_rows.size(), N = h->h_sr_node_off.back(), T = h->h_sr_task_off.back();
+  if (!out->node_off || !out->task_off || (Ns && !out->step_row) ||
+      (N && (!out->alloc_node || !out->alloc_ntasks || !out->alloc_res)) || (T && (!out->task_node || !out->task_res)))
+    return fail(h, CRANE_EINVAL, "step results: null column");
+  CU(cudaSetDevice(h->device));
+  cudaStream_t sm = h->stream;
+  if (Ns) memcpy(out->step_row, h->h_sr_rows.data(), Ns * sizeof(uint32_t));
+  memcpy(out->node_off, h->h_sr_node_off.data(), (Ns + 1) * sizeof(uint32_t));
+  memcpy(out->task_off, h->h_sr_task_off.data(), (Ns + 1) * sizeof(uint32_t));
+  if (N) {
+    CU(cudaMemcpyAsync(out->alloc_node, h->d_sa_node.p + h->sr_sa_base, N * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->alloc_res, h->d_sa_res.p + h->sr_sa_base, N * sizeof(Row), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->alloc_ntasks, h->d_sr_u32.p, N * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+  }
+  if (T) {
+    CU(cudaMemcpyAsync(out->task_node, h->d_sr_u32.p + N, T * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->task_res, h->d_sr_rows.p, T * sizeof(Row), cudaMemcpyDeviceToHost, sm));
+  }
+  CU(cudaStreamSynchronize(sm));
+  return CRANE_OK;
+}
+
+int crane_sched_step_jobs_avail(crane_sched_t* h, const uint32_t* rows, uint32_t n, crane_res_in_node_t* dst,
+                                uint32_t* n_node_rows) {
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "step_jobs_avail"));
+  TRY(check_rows(h, "step_jobs_avail", rows, n, h->n_sj, [&](uint32_t r) { return h->h_sj_dead[r] != 0; }));
+  std::vector<uint32_t> u(rows, rows + n);  // rows | dst_off
+  u.push_back(0);
+  for (uint32_t k = 0; k < n; ++k) u.push_back(u.back() + h->h_sj_node_off[rows[k] + 1] - h->h_sj_node_off[rows[k]]);
+  const uint32_t E = u.back();
+  if (n_node_rows) *n_node_rows = E;
+  CU(cudaSetDevice(h->device));
+  h->sp_results = false;
+  if (!E || !dst) return CRANE_OK;
+  H2D(h->d_sp_call, u.data(), u.size());
+  CU(h->d_sq_rows.ensure(E));
+  CRANE_LAUNCH(k_sj_avail_gather, warp_grid(h, n), 256, 0, h->stream, h->d_sj_node_off.p, h->d_sj_avail.p,
+               h->d_sp_call.p, h->d_sp_call.p + n, n, h->d_sq_rows.p);
+  CU(cudaMemcpyAsync(dst, h->d_sq_rows.p, (size_t)E * sizeof(Row), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  CU(cudaGetLastError());
   return CRANE_OK;
 }
 

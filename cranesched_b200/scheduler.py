@@ -102,6 +102,24 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.crane_sched_schedule_steps.restype = C.c_int
     lib.crane_sched_schedule_steps.argtypes = [C.c_void_p, P(abi.StepJobsC), P(abi.StepsC), P(abi.StepPlacementsC),
                                                P(C.c_float)]
+    lib.crane_sched_step_jobs_start.restype = C.c_int
+    lib.crane_sched_step_jobs_start.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, P(C.c_uint32)]
+    lib.crane_sched_step_jobs_append.restype = C.c_int
+    lib.crane_sched_step_jobs_append.argtypes = [C.c_void_p, P(abi.StepJobsC), P(C.c_uint32)]
+    lib.crane_sched_step_jobs_erase.restype = C.c_int
+    lib.crane_sched_step_jobs_erase.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    lib.crane_sched_steps_append.restype = C.c_int
+    lib.crane_sched_steps_append.argtypes = [C.c_void_p, P(abi.StepsC), C.c_void_p, P(C.c_uint32)]
+    lib.crane_sched_steps_erase.restype = C.c_int
+    lib.crane_sched_steps_erase.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    lib.crane_sched_steps_run.restype = C.c_int
+    lib.crane_sched_steps_run.argtypes = [C.c_void_p, P(C.c_uint32), P(C.c_uint32), P(C.c_uint32), P(C.c_float)]
+    lib.crane_sched_steps_fetch.restype = C.c_int
+    lib.crane_sched_steps_fetch.argtypes = [C.c_void_p, P(abi.StepResultsC)]
+    lib.crane_sched_step_jobs_avail.restype = C.c_int
+    lib.crane_sched_step_jobs_avail.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, P(C.c_uint32)]
+    lib.crane_sched_step_jobs_reset.restype = C.c_int
+    lib.crane_sched_step_jobs_reset.argtypes = [C.c_void_p]
     _libs[path] = lib
     return lib
 
@@ -114,7 +132,9 @@ EXPORTS = ("crane_sched_create", "crane_sched_destroy", "crane_sched_last_error"
            "crane_sched_qos_filter", "crane_sched_set_shard", "crane_sched_device_placements",
            "crane_sched_debug_bitmap", "crane_sched_debug_profile", "crane_sched_schedule_steps",
            "crane_sched_pending_set_gate", "crane_sched_pending_depend", "crane_sched_pending_cancel",
-           "crane_sched_running_end")
+           "crane_sched_running_end", "crane_sched_step_jobs_start", "crane_sched_step_jobs_append",
+           "crane_sched_step_jobs_erase", "crane_sched_steps_append", "crane_sched_steps_erase", "crane_sched_steps_run",
+           "crane_sched_steps_fetch", "crane_sched_step_jobs_avail", "crane_sched_step_jobs_reset")
 
 
 class GpuScheduler:
@@ -295,6 +315,64 @@ class GpuScheduler:
         c_j, c_s, c_o, ms = jobs.as_c(), steps.as_c(), out.as_c(), C.c_float(0.0)
         self._check(self._lib.crane_sched_schedule_steps(self._h, C.byref(c_j), C.byref(c_s), C.byref(c_o), C.byref(ms)))
         return out, ms.value
+
+    # --- the step state of running jobs kept resident on the device -------------------
+    def step_jobs_start(self, running_rows) -> int:
+        """Running rows become step jobs whose avail is their allocation
+        (SetStepResAvail, JobScheduler.cpp:1277); returns the first new step-job row."""
+        r = np.ascontiguousarray(running_rows, np.uint32)
+        first = C.c_uint32(0)
+        self._check(self._lib.crane_sched_step_jobs_start(self._h, r.ctypes.data, len(r), C.byref(first)))
+        return first.value
+
+    def step_jobs_append(self, jobs: abi.StepJobs) -> int:
+        """Step jobs from host rows (a crun primary, a job started elsewhere, recovery);
+        jobs.step_off is not sent. Returns the first new step-job row."""
+        c, first = jobs.as_c(), C.c_uint32(0)
+        c.step_off = None
+        self._check(self._lib.crane_sched_step_jobs_append(self._h, C.byref(c), C.byref(first)))
+        return first.value
+
+    def step_jobs_erase(self, rows):
+        """Jobs that left the running map: they and their steps go, nothing is released."""
+        r = np.ascontiguousarray(rows, np.uint32)
+        self._check(self._lib.crane_sched_step_jobs_erase(self._h, r.ctypes.data, len(r)))
+
+    def steps_append(self, steps: abi.Steps, job_row) -> int:
+        """AddStep: pending steps at the tail of their jobs' queues; returns the first new step row."""
+        j = np.ascontiguousarray(job_row, np.uint32)
+        if len(j) != steps.n:
+            raise ValueError("steps_append: one job row per step")
+        c, first = steps.as_c(), C.c_uint32(0)
+        self._check(self._lib.crane_sched_steps_append(self._h, C.byref(c), j.ctypes.data, C.byref(first)))
+        return first.value
+
+    def steps_erase(self, rows):
+        """EraseStep: pending rows leave their queue, scheduled rows give their allocation back."""
+        r = np.ascontiguousarray(rows, np.uint32)
+        self._check(self._lib.crane_sched_steps_erase(self._h, r.ctypes.data, len(r)))
+
+    def steps_run(self) -> tuple[abi.StepResults, float]:
+        """One pass of the step scheduler over the resident tables, then its results.
+        Returns (results, device ms of the pass's kernels)."""
+        n, nr, tr, ms = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0), C.c_float(0.0)
+        self._check(self._lib.crane_sched_steps_run(self._h, C.byref(n), C.byref(nr), C.byref(tr), C.byref(ms)))
+        out = abi.StepResults.sized(n.value, nr.value, tr.value)
+        c = out.as_c()
+        self._check(self._lib.crane_sched_steps_fetch(self._h, C.byref(c)))
+        return out, ms.value
+
+    def step_jobs_avail(self, rows) -> np.ndarray:
+        """The avail rows of step jobs `rows`, one job after another."""
+        r = np.ascontiguousarray(rows, np.uint32)
+        n = C.c_uint32(0)
+        self._check(self._lib.crane_sched_step_jobs_avail(self._h, r.ctypes.data, len(r), None, C.byref(n)))
+        dst = np.zeros(n.value, abi.RES_IN_NODE)
+        self._check(self._lib.crane_sched_step_jobs_avail(self._h, r.ctypes.data, len(r), dst.ctypes.data, None))
+        return dst
+
+    def step_jobs_reset(self):
+        self._check(self._lib.crane_sched_step_jobs_reset(self._h))
 
     def timing(self) -> dict:
         t = abi.TimingC()

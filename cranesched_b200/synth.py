@@ -635,26 +635,39 @@ def step_case(seed, select, base=None, max_steps=6, one_type_per_name=False, **c
     node or the task request, steps that take the whole allocation, steps that cannot
     fit (so later steps that would fit stay pending), and homogeneous requests whose
     equal task counts tie in the heap."""
-    from .abi import StepJobs, Steps
+    from .abi import StepJobs
     if base is None:
         base = random_case(seed, ntpn_range=True, one_type_per_name=one_type_per_name, **case_kw)
     cfg, cluster, running, pending, now = base
     node_off, node, avail = started_jobs(pending, select(cfg, cluster, running, pending, now))
     rng = np.random.Generator(np.random.PCG64(seed ^ 0x57E9))
-    names = np.array(list(cluster.gres_entry_name) + [0] * (GRES_ENTRIES - cluster.n_gres_entries))
     n_jobs = len(node_off) - 1
-    cols = {k: [] for k in ("node_num", "ntasks", "tmin", "tmax")}
-    req_node, req_task, incl, excl = [], [], [[0], []], [[0], []]
-    step_off = [0]
     n_steps = rng.integers(0, max_steps + 1, n_jobs)
+    draw = _StepDraw(cluster)
     for j in range(n_jobs):
-        k0, k1 = int(node_off[j]), int(node_off[j + 1])
-        nk = k1 - k0
-        a = avail[k0:k1]
+        draw.job(rng, node[node_off[j]:node_off[j + 1]], avail[node_off[j]:node_off[j + 1]], int(n_steps[j]))
+    jobs = StepJobs(node_off, node, avail, np.array(draw.step_off, np.uint32))
+    return cluster, jobs, draw.steps()
+
+
+class _StepDraw:
+    """The step draw of step_case: steps appended job by job (`job` draws `n` steps for a
+    job with nodes `node` and avail rows `a`), as one Steps table."""
+
+    def __init__(self, cluster):
+        self.cluster = cluster
+        self.names = np.array(list(cluster.gres_entry_name) + [0] * (GRES_ENTRIES - cluster.n_gres_entries))
+        self.cols = {k: [] for k in ("node_num", "ntasks", "tmin", "tmax")}
+        self.req_node, self.req_task, self.incl, self.excl = [], [], [[0], []], [[0], []]
+        self.step_off = [0]
+
+    def job(self, rng, node, a, n):
+        cluster, names, incl, excl = self.cluster, self.names, self.incl, self.excl
+        nk = len(node)
         cpu_min, mem_min = int(a["cpu_raw"].min()), int(a["mem"].min())
         gres_any = np.bitwise_or.reduce(a["gres"], axis=0) if nk else np.zeros(GRES_ENTRIES, np.uint16)
         ents = [e for e in range(cluster.n_gres_entries) if gres_any[e]]
-        for _ in range(int(n_steps[j])):
+        for _ in range(n):
             vn, vt = np.zeros((), RES_VIEW), np.zeros((), RES_VIEW)
             kind = rng.random()
             if kind < 0.12:  # the whole allocation: one task per node, everything the smallest node holds
@@ -689,22 +702,41 @@ def step_case(seed, select, base=None, max_steps=6, one_type_per_name=False, **c
                     if rng.random() < 0.5:
                         v["gres_spec"][e] += 1
             if rng.random() < 0.12:  # include list: a subset of the job's nodes, maybe an unknown host / outsider
-                sub = sorted(rng.choice(node[k0:k1], int(rng.integers(1, nk + 1)), replace=False).tolist())
+                sub = sorted(rng.choice(node, int(rng.integers(1, nk + 1)), replace=False).tolist())
                 if rng.random() < 0.3:
                     sub.append(0xFFFFFFFF if rng.random() < 0.5 else int(rng.integers(0, cluster.n_nodes)))
                 incl[1] += sub
             incl[0].append(len(incl[1]))
             if rng.random() < 0.12:
-                excl[1] += sorted(rng.choice(node[k0:k1], int(rng.integers(1, nk + 1)), replace=False).tolist())
+                excl[1] += sorted(rng.choice(node, int(rng.integers(1, nk + 1)), replace=False).tolist())
             excl[0].append(len(excl[1]))
-            for k, v in zip(cols, (nn, ntasks, tmin, tmax)):
-                cols[k].append(v)
-            req_node.append(vn)
-            req_task.append(vt)
-        step_off.append(len(cols["node_num"]))
-    jobs = StepJobs(node_off, node, avail, np.array(step_off, np.uint32))
-    steps = Steps(cols["node_num"], cols["ntasks"], cols["tmin"], cols["tmax"],
-                  np.array(req_node, RES_VIEW).reshape(-1), np.array(req_task, RES_VIEW).reshape(-1),
-                  np.array(incl[0], np.uint32), np.array(incl[1], np.uint32),
-                  np.array(excl[0], np.uint32), np.array(excl[1], np.uint32))
-    return cluster, jobs, steps
+            for k, v in zip(self.cols, (nn, ntasks, tmin, tmax)):
+                self.cols[k].append(v)
+            self.req_node.append(vn)
+            self.req_task.append(vt)
+        self.step_off.append(len(self.cols["node_num"]))
+
+    def steps(self):
+        from .abi import Steps
+        c, incl, excl = self.cols, self.incl, self.excl
+        return Steps(c["node_num"], c["ntasks"], c["tmin"], c["tmax"],
+                     np.array(self.req_node, RES_VIEW).reshape(-1), np.array(self.req_task, RES_VIEW).reshape(-1),
+                     np.array(incl[0], np.uint32), np.array(incl[1], np.uint32),
+                     np.array(excl[0], np.uint32), np.array(excl[1], np.uint32))
+
+
+def step_pass_stream(seed, node_off, node, avail, job_ids, cluster, max_steps=3, p_job=0.3):
+    """Step arrivals of one pass of the step scheduler over the jobs `job_ids` (indices
+    into the CSR node_off / node / avail: a job's nodes and its allocation, which sizes
+    its steps as in step_case): each job gets 1..max_steps new steps with probability
+    p_job, drawn by step_case's draw. Returns (job index of each new step, Steps)."""
+    rng = np.random.Generator(np.random.PCG64(seed ^ 0x5A55))
+    draw = _StepDraw(cluster)
+    owner = []
+    for j in job_ids:
+        if rng.random() >= p_job:
+            continue
+        n = int(rng.integers(1, max_steps + 1))
+        draw.job(rng, node[node_off[j]:node_off[j + 1]], avail[node_off[j]:node_off[j + 1]], n)
+        owner += [int(j)] * n
+    return np.array(owner, np.int64), draw.steps()

@@ -582,6 +582,87 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jobs,
                                const crane_steps_t* steps, crane_step_placements_t* out,
                                float* device_ms);
 
+/* ---- the step state of running jobs kept resident on the device ------------ */
+/* The daemon's step state changes by small events; these calls keep it on the device
+ * across passes of the step scheduler thread (JobScheduler.cpp:1637-1665) instead of
+ * re-sending every job with pending steps to crane_sched_schedule_steps on every pass.
+ * Two tables whose rows keep their index until crane_sched_step_jobs_reset (which is
+ * also how a caller compacts their tombstones: reset, then re-append the live rows):
+ *   step jobs  one row per running job that can get steps: its nodes (ascending and
+ *              distinct) and one step_res_avail_ row per node. Independent of the running
+ *              table: set_running, running_erase / running_end, set_cluster and every
+ *              NodeSelect call leave it alone.
+ *   steps      one row per step, bound to a step-job row, holding its crane_steps_t
+ *              columns; pending, scheduled or erased. A scheduled row keeps its node rows
+ *              (node, res) on the device so that erasing it gives them back. A job's FIFO
+ *              queue is its live pending step rows in row order.
+ * Daemon call sites:
+ *   job start, SetStepResAvail(allocated_res) (JobScheduler.cpp:1277), batch and calloc
+ *     primaries                     step_jobs_start(running rows): copies the running
+ *                                   rows' allocation entries into new step-job rows, on
+ *                                   the device
+ *   crun primary (InitPrimaryStepFromJob takes from avail on the host), a job started
+ *     elsewhere, a recovered job    step_jobs_append(host rows; step_off must be NULL)
+ *   AddStep (CtldPublicDefs.h:984)  steps_append(steps, job_row[n])
+ *   EraseStep (CtldPublicDefs.h:1000) steps_erase: a pending row leaves its queue; a
+ *                                   scheduled row's node rows are added back to its
+ *                                   job's avail (ResourceInNodeV3 +=)
+ *   job leaves m_running_job_map_   step_jobs_erase: the job and all its step rows go,
+ *                                   nothing is released
+ *   one pass of StepScheduleThread_ steps_run, then steps_fetch
+ * Rules:
+ *   - every call needs crane_sched_set_cluster (the gres dictionary);
+ *   - steps_append gives exactly the CRANE_EINVAL / CRANE_ENOSYS answers
+ *     crane_sched_schedule_steps gives for the same step, and CRANE_EINVAL for a job row
+ *     out of range or erased;
+ *   - step_jobs_start: CRANE_EINVAL for a running row out of range, erased, listed
+ *     twice, or whose allocation nodes are not ascending and distinct (rows that
+ *     crane_sched_start made always pass; rows of running_append may not, which a flag
+ *     on the device reports);
+ *   - every erase: CRANE_EINVAL for a row out of range, already erased, listed twice, or
+ *     whose job was erased; a refused call changes nothing;
+ *   - a pass visits only the jobs that are dirty and have a live pending step. A job
+ *     becomes dirty when it is appended or started, gets a step, loses a pending step or
+ *     gets an allocation back; every pass clears the flag. This is exact: after a pass
+ *     every job with pending steps is blocked at its head, and a job whose avail and
+ *     queue did not change would be blocked at the same head again;
+ *   - steps_run returns the number of steps it scheduled and of their node and task
+ *     rows, which size the caller's buffers; steps_fetch returns only those steps, step
+ *     rows ascending, in the layout of crane_step_placements_t (node rows in node-index
+ *     order, task rows in task-id order, node_off / task_off prefix sums over the
+ *     returned steps). Every later step call voids the fetch;
+ *   - no step call changes what NodeSelect reads or writes: the handle's stage (a
+ *     crane_sched_start after fetch / qos_filter still works with step calls in
+ *     between), the running table's regroup and the pending / running buffers;
+ *   - single caller, as every call on the handle: in the daemon both scheduler threads
+ *     hold m_running_job_map_mtx_ at their call sites (JobScheduler.cpp:1641).
+ * *first (optional) receives the first new row of an append or start; *device_ms
+ * (optional) the CUDA-event time of the pass's kernels. */
+typedef struct crane_step_results {
+  uint32_t* step_row;      /* [n_scheduled] step rows, ascending                       */
+  uint32_t* node_off;      /* [n_scheduled+1]                                          */
+  uint32_t* alloc_node;    /* [n_node_rows]                                            */
+  uint32_t* alloc_ntasks;  /* [n_node_rows]                                            */
+  crane_res_in_node_t* alloc_res; /* [n_node_rows]                                     */
+  uint32_t* task_off;      /* [n_scheduled+1]                                          */
+  uint32_t* task_node;     /* [n_task_rows]                                            */
+  crane_res_in_node_t* task_res;  /* [n_task_rows]                                     */
+} crane_step_results_t;
+
+int crane_sched_step_jobs_start(crane_sched_t* h, const uint32_t* running_rows, uint32_t n, uint32_t* first);
+int crane_sched_step_jobs_append(crane_sched_t* h, const crane_step_jobs_t* jobs, uint32_t* first);
+int crane_sched_step_jobs_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n);
+int crane_sched_steps_append(crane_sched_t* h, const crane_steps_t* steps, const uint32_t* job_row, uint32_t* first);
+int crane_sched_steps_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n);
+int crane_sched_steps_run(crane_sched_t* h, uint32_t* n_scheduled, uint32_t* n_node_rows, uint32_t* n_task_rows,
+                          float* device_ms);
+int crane_sched_steps_fetch(crane_sched_t* h, crane_step_results_t* out);
+/* The avail rows of step jobs rows[k], one job after another, into dst (host; NULL =
+ * only count them); *n_node_rows (optional) receives their number. */
+int crane_sched_step_jobs_avail(crane_sched_t* h, const uint32_t* rows, uint32_t n, crane_res_in_node_t* dst,
+                                uint32_t* n_node_rows);
+int crane_sched_step_jobs_reset(crane_sched_t* h);
+
 /* Capability bitmap of the last run (the jobs x nodes feasibility bitmap):
  * bit (rank r, local node q) set iff the r-th job in priority order can run
  * on the q-th node of its partition by total resources and node lists
