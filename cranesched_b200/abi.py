@@ -34,6 +34,7 @@ REASON_BEGIN_TIME = 8
 REASON_DEPENDENCY = 9
 REASON_DEPENDENCY_NEVER = 10
 REASON_ERASED = 255  # a row removed from the device-resident pending table
+ROW_NONE = 0xFFFFFFFF  # crane_sched_compact: the map entry of an erased row
 REASON_QOS_CPU = 16
 REASON_QOS_JOBS = 17
 REASON_QOS_WALL = 18

@@ -13,7 +13,7 @@ CSRC = os.path.join(ROOT, "cranesched_b200", "csrc")
 SO = os.path.join(CSRC, "libcrane_sched.so")
 EMU_SO = os.path.join(ROOT, "tests", "_emu", "libcrane_sched_emu.so")
 _SOURCES = ["sched_api.cu", "sched_kernels.cuh", "commit_v2.cuh", "qos_kernels.cuh", "step_kernels.cuh", "running_kernels.cuh",
-            "gate_kernels.cuh", "step_resident_kernels.cuh", "algebra.cuh"]
+            "gate_kernels.cuh", "step_resident_kernels.cuh", "compact_kernels.cuh", "algebra.cuh"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 
 

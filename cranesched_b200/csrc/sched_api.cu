@@ -33,6 +33,7 @@
 #include "running_kernels.cuh"
 #include "gate_kernels.cuh"
 #include "step_resident_kernels.cuh"
+#include "compact_kernels.cuh"
 
 using namespace crane;
 
@@ -75,6 +76,15 @@ struct DBuf {
     p = q;
     cap = want;
     return e;
+  }
+  void swap(DBuf& o) {
+    std::swap(p, o.p);
+    std::swap(cap, o.cap);
+  }
+  void release() {
+    if (p) cudaFree(p);
+    p = nullptr;
+    cap = 0;
   }
 };
 
@@ -1422,6 +1432,273 @@ int crane_sched_running_end(crane_sched_t* h, const uint32_t* rows, uint32_t n, 
   ev.code = h->d_ev_u32.p;
   TRY(dep_fire(h, ev, n, h->n_ent));
   CU(cudaStreamSynchronize(h->stream));
+  return CRANE_OK;
+}
+
+}  // extern "C" (the compaction's helpers live in an unnamed namespace)
+
+namespace {
+
+// The live rows of a table of n rows, in row order (the stable sort by tombstone flag),
+// into live[0, n_live), and the old -> new map into map[0, n)
+int live_rows(crane_sched* h, const uint8_t* dead, uint32_t n, uint32_t n_live, uint32_t* live, uint32_t* map) {
+  cudaStream_t st = h->stream;
+  uint64_t* keys;
+  uint32_t* vals;
+  CRANE_LAUNCH(k_rt_live_keys, (n + 255) / 256, 256, 0, st, dead, n, h->d_keys_a.p, h->d_vals_a.p);
+  TRY(radix_sort(h, n, 8, &keys, &vals));
+  if (n_live) CU(cudaMemcpyAsync(live, vals, sizeof(uint32_t) * n_live, cudaMemcpyDeviceToDevice, st));
+  CU(cudaMemsetAsync(map, 0xff, sizeof(uint32_t) * n, st));
+  if (n_live) CRANE_LAUNCH(k_cp_map, (n_live + 255) / 256, 256, 0, st, live, n_live, map);
+  return CRANE_OK;
+}
+
+// new_off[0, n_live] = the offsets of the live rows of a CSR table
+int csr_offsets(crane_sched* h, const uint32_t* off, const uint32_t* live, uint32_t n_live, uint32_t* new_off) {
+  CRANE_LAUNCH(k_cp_lengths, (n_live + 1 + 255) / 256, 256, 0, h->stream, off, live, n_live, new_off);
+  CRANE_LAUNCH(k_sort_scan, 1, 1024, 0, h->stream, new_off, n_live + 1);
+  return CRANE_OK;
+}
+
+// The entries of the live rows of a CSR table at their new offsets
+template <class T>
+int csr_copy(crane_sched* h, const uint32_t* off, const T* src, const uint32_t* live, uint32_t n_live,
+             const uint32_t* new_off, T* dst) {
+  if (!n_live) return CRANE_OK;
+  const uint32_t nb = std::min<uint32_t>((n_live + 7) / 8, 8 * h->n_sm);
+  CRANE_LAUNCH(k_cp_csr<T>, nb, 256, 0, h->stream, off, src, live, n_live, new_off, dst);
+  return CRANE_OK;
+}
+
+// Host mirror of a CSR table's offsets for its live rows
+std::vector<uint32_t> live_offsets(const std::vector<uint32_t>& off, const std::vector<uint8_t>& dead) {
+  std::vector<uint32_t> o(1, 0);
+  for (size_t r = 0; r < dead.size(); ++r)
+    if (!dead[r]) o.push_back(o.back() + (off[r + 1] - off[r]));
+  return o;
+}
+
+template <class T>
+std::vector<T> live_only(const std::vector<T>& v, const std::vector<uint8_t>& dead) {
+  std::vector<T> o;
+  for (size_t r = 0; r < dead.size(); ++r)
+    if (!dead[r]) o.push_back(v[r]);
+  return o;
+}
+
+}  // namespace
+
+extern "C" {
+
+int crane_sched_compact(crane_sched_t* h, uint32_t* pending_map, uint32_t* running_map) {
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "compact"));
+  CU(cudaSetDevice(h->device));
+  lower_stage(h, kCluster);  // the run's outputs are indexed by the old rows
+  cudaStream_t st = h->stream;
+  const uint32_t N = h->n_pending, Rt = h->n_rr, M = h->n_ent;
+  const bool cp_pd = h->n_dead > 0, cp_rr = h->n_rr_dead > 0;
+  const uint32_t Nl = N - h->n_dead, Rl = Rt - h->n_rr_dead;
+  uint32_t gate_n = 0;  // rows of the new table with gate state: the live rows below gate_n
+  for (uint32_t r = 0; r < h->gate_n; ++r) gate_n += h->h_dead[r] ? 0 : 1;
+
+  // ---- work buffers, then the live rows, the maps and the open entries ----
+  const size_t ns = std::max<size_t>({(size_t)N, (size_t)Rt, (size_t)M, 1});
+  CU(h->d_keys_a.ensure(ns));
+  CU(h->d_keys_b.ensure(ns));
+  CU(h->d_vals_a.ensure(ns));
+  CU(h->d_vals_b.ensure(ns));
+  CU(h->d_flag.ensure(1));
+  DBuf<uint32_t> pd_live, pd_map, rr_live, rr_map, keep;
+  if (cp_pd) {
+    CU(pd_live.ensure(std::max<uint32_t>(Nl, 1)));
+    CU(pd_map.ensure(N));
+    TRY(live_rows(h, h->d_dead.p, N, Nl, pd_live.p, pd_map.p));
+  }
+  if (cp_rr) {
+    CU(rr_live.ensure(std::max<uint32_t>(Rl, 1)));
+    CU(rr_map.ensure(Rt));
+    TRY(live_rows(h, h->d_rr_dead.p, Rt, Rl, rr_live.p, rr_map.p));
+  }
+  uint32_t n_keep = 0;
+  if (M) {
+    CU(keep.ensure(M));
+    CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
+    CRANE_LAUNCH(k_cp_ent_keys, (M + 255) / 256, 256, 0, st, gate_dev(h), h->n_dead ? h->d_dead.p : nullptr,
+                 h->d_keys_a.p, h->d_vals_a.p, h->d_flag.p);
+    uint64_t* keys;
+    uint32_t* vals;
+    TRY(radix_sort(h, M, 8, &keys, &vals));
+    CU(cudaMemcpyAsync(keep.p, vals, sizeof(uint32_t) * M, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(&n_keep, h->d_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  const bool cp_ent = M && (n_keep < M || cp_pd || cp_rr);
+
+  // ---- every new buffer before the first gather: CRANE_ENOMEM leaves the tables as they were ----
+  std::vector<uint32_t> alloc_off, incl_off, excl_off, rr_alloc_off;
+  DBuf<uint32_t> partition, node_num, ntpn, ntpn_max, ntasks, part_prio, qos_prio, account, qos, user, pd_resv,
+      p_alloc_off, p_incl_off, p_incl_nodes, p_excl_off, p_excl_nodes, g_open;
+  DBuf<int64_t> time_limit, submit, g_begin;
+  DBuf<uint8_t> exclusive, dead, g_held, g_is_or;
+  DBuf<double> mandated;
+  DBuf<View> req_node, req_task, req_total;
+  DBuf<long long> g_ready;
+  if (cp_pd) {
+    const size_t n1 = std::max<uint32_t>(Nl, 1);
+    alloc_off = live_offsets(h->h_alloc_off, h->h_dead);
+    CU(partition.ensure(n1)); CU(time_limit.ensure(n1)); CU(submit.ensure(n1)); CU(node_num.ensure(n1));
+    CU(ntpn.ensure(n1)); CU(ntpn_max.ensure(n1)); CU(ntasks.ensure(n1)); CU(exclusive.ensure(n1));
+    CU(part_prio.ensure(n1)); CU(qos_prio.ensure(n1)); CU(account.ensure(n1));
+    CU(req_node.ensure(n1)); CU(req_task.ensure(n1)); CU(req_total.ensure(n1));
+    CU(dead.ensure(n1));
+    CU(p_alloc_off.ensure(n1 + 1));
+    if (h->have_qos_cols) { CU(qos.ensure(n1)); CU(user.ensure(n1)); }
+    if (h->have_mandated) CU(mandated.ensure(n1));
+    if (h->have_pd_resv) CU(pd_resv.ensure(n1));
+    if (h->have_lists_incl) {
+      incl_off = live_offsets(h->h_incl_off, h->h_dead);
+      CU(p_incl_off.ensure(n1 + 1));
+      CU(p_incl_nodes.ensure(std::max<uint32_t>(incl_off.back(), 1)));
+    }
+    if (h->have_lists_excl) {
+      excl_off = live_offsets(h->h_excl_off, h->h_dead);
+      CU(p_excl_off.ensure(n1 + 1));
+      CU(p_excl_nodes.ensure(std::max<uint32_t>(excl_off.back(), 1)));
+    }
+    if (h->gate_n) {
+      const size_t g1 = std::max<uint32_t>(gate_n, 1);
+      CU(g_held.ensure(g1)); CU(g_begin.ensure(g1)); CU(g_is_or.ensure(g1)); CU(g_open.ensure(g1)); CU(g_ready.ensure(g1));
+    }
+  }
+  DBuf<int64_t> rr_start, rr_end, rr_cpu;
+  DBuf<uint32_t> rr_node_num, rr_part_prio, rr_qos_prio, rr_account, rr_resv, r_alloc_off, rr_alloc_node;
+  DBuf<uint64_t> rr_mem;
+  DBuf<Row> rr_alloc_res;
+  DBuf<uint8_t> rr_dead;
+  if (cp_rr) {
+    const size_t r1 = std::max<uint32_t>(Rl, 1);
+    rr_alloc_off = live_offsets(h->h_rr_alloc_off, h->h_rr_dead);
+    CU(rr_start.ensure(r1)); CU(rr_end.ensure(r1)); CU(rr_cpu.ensure(r1)); CU(rr_node_num.ensure(r1));
+    CU(rr_part_prio.ensure(r1)); CU(rr_qos_prio.ensure(r1)); CU(rr_account.ensure(r1)); CU(rr_resv.ensure(r1));
+    CU(rr_mem.ensure(r1)); CU(rr_dead.ensure(r1));
+    CU(r_alloc_off.ensure(r1 + 1));
+    CU(rr_alloc_node.ensure(std::max<uint32_t>(rr_alloc_off.back(), 1)));
+    CU(rr_alloc_res.ensure(std::max<uint32_t>(rr_alloc_off.back(), 1)));
+  }
+  DBuf<uint32_t> e_dependent, e_dependee;
+  DBuf<uint8_t> e_kind, e_type, e_live;
+  DBuf<uint64_t> e_delay;
+  if (cp_ent) {
+    const size_t m1 = std::max<uint32_t>(n_keep, 1);
+    CU(e_dependent.ensure(m1)); CU(e_dependee.ensure(m1)); CU(e_kind.ensure(m1)); CU(e_type.ensure(m1));
+    CU(e_live.ensure(m1)); CU(e_delay.ensure(m1));
+  }
+
+  // ---- gathers ----
+  if (cp_pd) {
+    PendingCols s{h->d_partition.p, h->d_time_limit.p, h->d_submit.p, h->d_node_num.p, h->d_ntpn.p, h->d_ntpn_max.p,
+                  h->d_ntasks.p, h->d_exclusive.p, h->d_part_prio.p, h->d_qos_prio.p, h->d_account.p, h->d_qos.p,
+                  h->d_user.p, h->d_mandated.p, h->d_pd_resv.p, h->d_req_node.p, h->d_req_task.p, h->d_req_total.p,
+                  h->d_g_held.p, h->d_g_begin.p, h->d_g_is_or.p, h->d_g_open.p, h->d_g_ready.p};
+    PendingCols d{partition.p, time_limit.p, submit.p, node_num.p, ntpn.p, ntpn_max.p, ntasks.p, exclusive.p,
+                  part_prio.p, qos_prio.p, account.p, qos.p, user.p, mandated.p, pd_resv.p, req_node.p, req_task.p,
+                  req_total.p, g_held.p, g_begin.p, g_is_or.p, g_open.p, g_ready.p};
+    if (Nl) CRANE_LAUNCH(k_cp_pending, (Nl + 255) / 256, 256, 0, st, s, d, pd_live.p, Nl, gate_n);
+    CU(cudaMemsetAsync(dead.p, 0, std::max<uint32_t>(Nl, 1), st));
+    TRY(csr_offsets(h, h->d_alloc_off.p, pd_live.p, Nl, p_alloc_off.p));
+    if (h->have_lists_incl) {
+      TRY(csr_offsets(h, h->d_incl_off.p, pd_live.p, Nl, p_incl_off.p));
+      TRY(csr_copy(h, h->d_incl_off.p, h->d_incl_nodes.p, pd_live.p, Nl, p_incl_off.p, p_incl_nodes.p));
+    }
+    if (h->have_lists_excl) {
+      TRY(csr_offsets(h, h->d_excl_off.p, pd_live.p, Nl, p_excl_off.p));
+      TRY(csr_copy(h, h->d_excl_off.p, h->d_excl_nodes.p, pd_live.p, Nl, p_excl_off.p, p_excl_nodes.p));
+    }
+  }
+  if (cp_rr) {
+    const RunTableDev s = run_table(h);
+    RunTableDev d{};
+    d.start_time = rr_start.p; d.end_time = rr_end.p; d.node_num = rr_node_num.p; d.partition_priority = rr_part_prio.p;
+    d.qos_priority = rr_qos_prio.p; d.account = rr_account.p; d.reservation = rr_resv.p; d.view_cpu_raw = rr_cpu.p;
+    d.view_mem = rr_mem.p;
+    if (Rl) CRANE_LAUNCH(k_cp_running, (Rl + 255) / 256, 256, 0, st, s, d, rr_live.p, Rl);
+    CU(cudaMemsetAsync(rr_dead.p, 0, std::max<uint32_t>(Rl, 1), st));
+    TRY(csr_offsets(h, s.alloc_off, rr_live.p, Rl, r_alloc_off.p));
+    TRY(csr_copy(h, s.alloc_off, s.alloc_node, rr_live.p, Rl, r_alloc_off.p, rr_alloc_node.p));
+    TRY(csr_copy(h, s.alloc_off, s.alloc_res, rr_live.p, Rl, r_alloc_off.p, rr_alloc_res.p));
+  }
+  if (cp_ent && n_keep) {
+    GateDev d = gate_dev(h);
+    d.dependent = e_dependent.p; d.dependee = e_dependee.p; d.kind = e_kind.p; d.type = e_type.p; d.live = e_live.p;
+    CRANE_LAUNCH(k_cp_entries, (n_keep + 255) / 256, 256, 0, st, gate_dev(h), d, e_delay.p, keep.p, n_keep,
+                 cp_pd ? pd_map.p : nullptr, cp_rr ? rr_map.p : nullptr);
+  }
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(st));
+
+  // ---- the new tables replace the old ones (whose buffers go with the locals) ----
+  if (cp_pd) {
+    h->d_partition.swap(partition); h->d_time_limit.swap(time_limit); h->d_submit.swap(submit);
+    h->d_node_num.swap(node_num); h->d_ntpn.swap(ntpn); h->d_ntpn_max.swap(ntpn_max); h->d_ntasks.swap(ntasks);
+    h->d_exclusive.swap(exclusive); h->d_part_prio.swap(part_prio); h->d_qos_prio.swap(qos_prio);
+    h->d_account.swap(account); h->d_req_node.swap(req_node); h->d_req_task.swap(req_task);
+    h->d_req_total.swap(req_total); h->d_dead.swap(dead); h->d_alloc_off.swap(p_alloc_off);
+    if (h->have_qos_cols) { h->d_qos.swap(qos); h->d_user.swap(user); }
+    if (h->have_mandated) h->d_mandated.swap(mandated);
+    if (h->have_pd_resv) h->d_pd_resv.swap(pd_resv);
+    if (h->have_lists_incl) { h->d_incl_off.swap(p_incl_off); h->d_incl_nodes.swap(p_incl_nodes); h->h_incl_off = incl_off; }
+    if (h->have_lists_excl) { h->d_excl_off.swap(p_excl_off); h->d_excl_nodes.swap(p_excl_nodes); h->h_excl_off = excl_off; }
+    if (h->gate_n) {
+      h->d_g_held.swap(g_held); h->d_g_begin.swap(g_begin); h->d_g_is_or.swap(g_is_or); h->d_g_open.swap(g_open);
+      h->d_g_ready.swap(g_ready);
+      h->h_has_deps = live_only(h->h_has_deps, std::vector<uint8_t>(h->h_dead.begin(), h->h_dead.begin() + h->gate_n));
+    }
+    h->h_alloc_off = alloc_off;
+    h->h_pd_account = live_only(h->h_pd_account, h->h_dead);
+    h->h_dead.assign(Nl, 0);
+    h->n_dead = 0;
+    h->n_pending = Nl;
+    h->total_alloc = alloc_off.back();
+    h->gate_n = gate_n;
+  }
+  if (cp_rr) {
+    h->d_rr_start.swap(rr_start); h->d_rr_end.swap(rr_end); h->d_rr_cpu.swap(rr_cpu); h->d_rr_node_num.swap(rr_node_num);
+    h->d_rr_part_prio.swap(rr_part_prio); h->d_rr_qos_prio.swap(rr_qos_prio); h->d_rr_account.swap(rr_account);
+    h->d_rr_resv.swap(rr_resv); h->d_rr_mem.swap(rr_mem); h->d_rr_dead.swap(rr_dead);
+    h->d_rr_alloc_off.swap(r_alloc_off); h->d_rr_alloc_node.swap(rr_alloc_node); h->d_rr_alloc_res.swap(rr_alloc_res);
+    h->h_rr_account = live_only(h->h_rr_account, h->h_rr_dead);
+    h->h_rr_alloc_off = rr_alloc_off;
+    h->h_rr_dead.assign(Rl, 0);
+    h->n_rr_dead = 0;
+    h->n_rr = Rl;
+    // (the run's view of the running table is the live rows in row order: rr_dirty stays)
+  }
+  if (cp_ent) {
+    h->d_e_dependent.swap(e_dependent); h->d_e_dependee.swap(e_dependee); h->d_e_kind.swap(e_kind);
+    h->d_e_type.swap(e_type); h->d_e_live.swap(e_live); h->d_e_delay.swap(e_delay);
+    h->n_ent = n_keep;
+  }
+  if (cp_pd || cp_rr) {
+    // work and output buffers sized for the old tables: keep_running sizes them again
+    h->d_keys_a.release(); h->d_keys_b.release(); h->d_vals_a.release(); h->d_vals_b.release();
+    h->d_prio.release(); h->d_g_code.release(); h->d_vpart.release(); h->d_jobq.release(); h->d_bitmap.release();
+    h->d_reason.release(); h->d_out_prio.release(); h->d_out_start.release(); h->d_out_end.release();
+    h->d_out_nalloc.release(); h->d_out_node.release(); h->d_out_ntasks.release(); h->d_out_res.release();
+    h->d_hist.release();
+  }
+
+  // ---- the maps ----
+  if (pending_map) {
+    if (cp_pd) CU(cudaMemcpyAsync(pending_map, pd_map.p, sizeof(uint32_t) * N, cudaMemcpyDeviceToHost, st));
+    else for (uint32_t r = 0; r < N; ++r) pending_map[r] = r;
+  }
+  if (running_map) {
+    if (cp_rr) CU(cudaMemcpyAsync(running_map, rr_map.p, sizeof(uint32_t) * Rt, cudaMemcpyDeviceToHost, st));
+    else for (uint32_t r = 0; r < Rt; ++r) running_map[r] = r;
+  }
+  CU(cudaStreamSynchronize(st));
   return CRANE_OK;
 }
 

@@ -120,6 +120,8 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.crane_sched_step_jobs_avail.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, P(C.c_uint32)]
     lib.crane_sched_step_jobs_reset.restype = C.c_int
     lib.crane_sched_step_jobs_reset.argtypes = [C.c_void_p]
+    lib.crane_sched_compact.restype = C.c_int
+    lib.crane_sched_compact.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     _libs[path] = lib
     return lib
 
@@ -134,7 +136,8 @@ EXPORTS = ("crane_sched_create", "crane_sched_destroy", "crane_sched_last_error"
            "crane_sched_pending_set_gate", "crane_sched_pending_depend", "crane_sched_pending_cancel",
            "crane_sched_running_end", "crane_sched_step_jobs_start", "crane_sched_step_jobs_append",
            "crane_sched_step_jobs_erase", "crane_sched_steps_append", "crane_sched_steps_erase", "crane_sched_steps_run",
-           "crane_sched_steps_fetch", "crane_sched_step_jobs_avail", "crane_sched_step_jobs_reset")
+           "crane_sched_steps_fetch", "crane_sched_step_jobs_avail", "crane_sched_step_jobs_reset",
+           "crane_sched_compact")
 
 
 class GpuScheduler:
@@ -272,6 +275,17 @@ class GpuScheduler:
         if len(t) != len(r) or len(c) != len(r):
             raise ValueError("running_end: one end time and one exit code per row")
         self._check(self._lib.crane_sched_running_end(self._h, r.ctypes.data, len(r), t.ctypes.data, c.ctypes.data))
+
+    def compact(self, maps: bool = True) -> tuple[np.ndarray | None, np.ndarray | None]:
+        """Drops the erased rows of the resident pending and running tables and the resolved
+        dependency entries, on the device. Returns (pending_map, running_map): uint32, the
+        new row of every old row or abi.ROW_NONE for an erased one (None, None when `maps`
+        is false: the call then passes NULL maps)."""
+        pm = np.zeros(self.pending_rows(), np.uint32) if maps else None
+        rm = np.zeros(self.running_rows(), np.uint32) if maps else None
+        self._check(self._lib.crane_sched_compact(self._h, None if pm is None else pm.ctypes.data,
+                                                  None if rm is None else rm.ctypes.data))
+        return pm, rm
 
     def run(self, now: int):
         self._check(self._lib.crane_sched_run(self._h, now))

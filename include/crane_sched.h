@@ -290,7 +290,7 @@ int crane_sched_fetch(crane_sched_t* h, crane_placements_t* out);
  * node_num over ALL rows); an erased row reports CRANE_REASON_ERASED and takes
  * part in nothing (priority bounds, batch limit, queue). Rows must arrive in
  * job-id order (equal priorities keep row order). crane_sched_upload ==
- * pending_reset; pending_append; set_running. Re-upload to compact. */
+ * pending_reset; pending_append; set_running. crane_sched_compact drops the erased rows. */
 int crane_sched_pending_reset(crane_sched_t* h);
 int crane_sched_pending_append(crane_sched_t* h, const crane_pending_t* rows, uint32_t* first_row);
 int crane_sched_pending_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n);
@@ -305,7 +305,7 @@ uint32_t crane_sched_pending_rows(const crane_sched_t* h);
  *     crane_sched_running_erase(h, ended, m);
  *     crane_sched_keep_running(h, NULL); crane_sched_run(h, now); crane_sched_fetch(h, out)
  * and uploads no job data. crane_sched_set_running == reset; running_append;
- * keep_running, which is also how a caller compacts the tombstones. Reservation
+ * keep_running; crane_sched_compact drops the tombstones in place. Reservation
  * indices of running rows follow crane_sched_set_reservations, as for pending rows.
  *
  * running_append: appends host rows (recovery at daemon start, jobs started
@@ -412,13 +412,43 @@ typedef struct crane_dependencies {
  * pending_cancel or running_end. crane_sched_set_running replaces the running table, so
  * entries waiting on running rows must be re-sent (pending_reset, pending_append,
  * set_gate, pending_depend with EVENT entries for what was resolved) when it is used to
- * compact a table with dependencies. */
+ * compact a table with dependencies; crane_sched_compact compacts with the dependency
+ * state in place and needs none of that. */
 int crane_sched_pending_set_gate(crane_sched_t* h, const uint32_t* rows, uint32_t n, const uint8_t* held,
                                  const int64_t* begin_time);
 int crane_sched_pending_depend(crane_sched_t* h, const crane_dependencies_t* deps);
 int crane_sched_pending_cancel(crane_sched_t* h, const uint32_t* rows, uint32_t n, int64_t cancel_time);
 int crane_sched_running_end(crane_sched_t* h, const uint32_t* rows, uint32_t n, const int64_t* end_time,
                             const uint32_t* exit_code);
+
+/* ---- compaction of the resident tables ------------------------------------------ */
+/* Erased rows and resolved dependency entries stay behind in the resident tables, and
+ * every run, fetch and dependency event pays for them. crane_sched_compact rewrites the
+ * pending and the running table and the dependency entries on the device, keeping only
+ * what is live:
+ *   pending table  erased rows go; gated rows (held, begin time ahead, dependencies open
+ *                  or never satisfiable) are live and stay. Live rows keep their relative
+ *                  order: the new index is the row's rank among the live rows, so job-id
+ *                  order still holds for later appends. pending_map[old] (pending_rows
+ *                  before the call) = the new row, or CRANE_ROW_NONE for an erased row.
+ *   running table  the same: running_map[old] (running_rows before the call).
+ *   entries        resolved entries and entries of erased rows go. A kept entry's rows
+ *                  follow the maps; its gate state (held, begin time, is_or, open entries,
+ *                  ready_time) moves with its row. An entry whose dependee row was erased
+ *                  without events (pending_erase / running_erase) never fires, before or
+ *                  after compaction.
+ * Either map may be NULL. Tables without erased rows or resolved entries stay as they are
+ * (identity maps); step tables are untouched (they name no pending or running row).
+ * Erased rows and resolved entries take part in nothing and the live rows keep their
+ * order, so the next run's outputs equal the uncompacted table's, byte for byte, at the
+ * mapped rows. Device memory drops to the live rows plus the usual headroom; the peak is
+ * the old tables plus the live copy, and CRANE_ENOMEM leaves the tables as they were.
+ * No job data crosses PCIe, only the maps. Call it after start / running_end /
+ * pending_cancel and before keep_running; it needs set_cluster and voids the last run,
+ * like pending_erase (fetch, start and qos_filter need keep_running and run again). On a
+ * sharded handle every rank makes the same call. When to compact is the caller's choice. */
+#define CRANE_ROW_NONE 0xFFFFFFFFu
+int crane_sched_compact(crane_sched_t* h, uint32_t* pending_map, uint32_t* running_map);
 
 /* Blocks until the handle's stream is idle; *run_ms (optional) receives the
  * device time of the last crane_sched_run (CUDA events on that stream). */
