@@ -425,6 +425,192 @@ def random_case(seed, n_jobs=300, n_nodes=48, n_parts=3, n_running=40, fifo=Fals
     return cfg, cluster, running, pend, NOW
 
 
+# ---------------------------------------------------------------------------
+# Cases at the kernels' size limits: many node shapes per partition, cores up to
+# 256 (not always a prefix), all eight gres entries with up to 16 slots, jobs
+# wider than a batch (32), than one re-key (64) and up to the general task
+# distribution's heap (127 nodes), running jobs holding high cores and slots.
+# ---------------------------------------------------------------------------
+EDGE_CORES = (8, 32, 64, 65, 96, 128, 129, 192, 255, 256)
+EDGE_WIDE = (31, 32, 33, 63, 64, 65, 100, 127)
+EDGE_SLOTS = (1, 2, 4, 8, 12, 16)
+
+
+def _bits_mask(bits, words):
+    m = [0] * words
+    for b in bits:
+        m[b // 64] |= 1 << (b % 64)
+    return m
+
+
+def _edge_shape(rng, k, n_entries):
+    """One res_total row; k (the shape's index) makes rows of different shapes distinct."""
+    cores = int(rng.choice(EDGE_CORES))
+    u = rng.random()
+    if u < 0.25 and cores < 256:  # a run of cores that does not start at 0
+        lo = int(rng.integers(1, 256 - cores + 1))
+        bits = range(lo, lo + cores)
+    elif u < 0.4:  # scattered over all four words
+        bits = rng.choice(256, cores, replace=False).tolist()
+    else:
+        bits = range(cores)
+    r = np.zeros((), RES_IN_NODE)
+    r["cpu_raw"] = cores * 256
+    r["mem"] = r["mem_sw"] = (64 + 8 * k) * GiB
+    r["core"] = np.array(_bits_mask(bits, CORE_WORDS), np.uint64)
+    for e in range(n_entries):
+        if rng.random() < 0.55:
+            n = int(rng.choice(EDGE_SLOTS))
+            slots = range(n) if rng.random() < 0.7 else rng.choice(16, n, replace=False).tolist()
+            r["gres"][e] = _bits_mask(slots, 1)[0]
+    return r
+
+
+def _first_bits(mask_words, width, k):
+    """The k lowest set bits of a mask given as `width`-bit words (first fit)."""
+    out = []
+    for w, v in enumerate(mask_words):
+        v = int(v)
+        while v and len(out) < k:
+            low = v & -v
+            out.append(w * width + low.bit_length() - 1)
+            v ^= low
+    return out
+
+
+def edge_case(seed, n_jobs=400, parts=((140, 20),), one_type_per_name=False, n_running=40,
+              wide=EDGE_WIDE, p_wide=0.1, p_general=0.4, p_full=0.01, p_down=0.04, fifo=False, cost_policy=0,
+              short=False, limit=None):
+    """A case at the kernels' size limits, in the (cfg, cluster, running, pending, now) form of the others.
+
+    parts: (nodes, distinct res_total rows) per partition, disjoint; every shape has at least one usable
+    node, so a partition's number of usable classes is exactly its shape count. Gres: eight entries, one
+    type per name (one_type_per_name, the layout the reference pin needs) or several types per name.
+    Jobs: mostly 1-3 nodes with `p_wide` of them as wide as `wide`, `p_full` as wide as their whole
+    partition; `p_general` of the jobs up to 127 nodes get a ntasks_per_node range and uneven ntasks.
+    `p_down` of the nodes are dead and as many drained.
+    Running jobs are carved first-fit from the node totals (high cores, entries 4-7), some ending inside
+    the backfill window. Multifactor priorities are all distinct (mandated): the reference's sort is
+    unstable."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    names = tuple(range(GRES_ENTRIES)) if one_type_per_name else (0, 0, 0, 1, 1, 1, 2, 2)
+    rows, alive, drain, off, sizes, k0 = [], [], [], [0], [], 0
+    for n, n_shapes in parts:
+        assert 1 <= n_shapes <= n
+        shapes = [_edge_shape(rng, k0 + k, GRES_ENTRIES) for k in range(n_shapes)]
+        k0 += n_shapes
+        pick = np.concatenate([np.arange(n_shapes), rng.integers(0, n_shapes, n - n_shapes)])
+        rng.shuffle(pick)
+        a = (rng.random(n) >= p_down).astype(np.uint8)
+        d = (rng.random(n) < p_down).astype(np.uint8)
+        for k in range(n_shapes):  # one usable node of every shape
+            first = int(np.flatnonzero(pick == k)[0])
+            a[first], d[first] = 1, 0
+        rows += [shapes[k] for k in pick]
+        alive.append(a)
+        drain.append(d)
+        sizes.append(n)
+        off.append(off[-1] + n)
+    res_total = np.array(rows, RES_IN_NODE)
+    n_nodes, n_parts = len(res_total), len(parts)
+    alive, drain = np.concatenate(alive), np.concatenate(drain)
+    cluster = Cluster(res_total, alive, drain, np.array(off, np.uint32), np.arange(n_nodes, dtype=np.uint32),
+                      len(names), names)
+    usable = [int(((alive == 1) & (drain == 0))[off[p]:off[p + 1]].sum()) for p in range(n_parts)]
+
+    # running jobs: first fit out of what is left on the node, cores of every word, slots of every entry
+    left = res_total.copy()
+    r_start, r_end, r_nn, r_cpu, r_mem, r_off, r_node, r_res = [], [], [], [], [], [0], [], []
+    for _ in range(n_running):
+        nn = int(rng.choice([1, 1, 1, 2, 3, 6]))
+        ok_nodes, rowsj = [], []
+        for nd in sorted(rng.choice(n_nodes, nn, replace=False).tolist()):
+            free = _first_bits(left[nd]["core"], 64, 256)
+            cores = int(rng.integers(1, 9)) if rng.random() < 0.5 else int(rng.integers(40, 200))
+            cores = min(cores, len(free) - 1)
+            mem = int(rng.integers(1, 17)) * GiB
+            if cores < 1 or int(left[nd]["mem"]) < mem:
+                continue
+            row = np.zeros((), RES_IN_NODE)
+            row["cpu_raw"] = cores * 256
+            row["core"] = np.array(_bits_mask(free[:cores], CORE_WORDS), np.uint64)
+            row["mem"] = row["mem_sw"] = mem
+            for e in range(GRES_ENTRIES):
+                have = _first_bits([left[nd]["gres"][e]], 16, 16)
+                if have and rng.random() < 0.5:
+                    row["gres"][e] = _bits_mask(have[:int(rng.integers(1, len(have) + 1))], 1)[0]
+            left[nd]["cpu_raw"] -= row["cpu_raw"]
+            left[nd]["mem"] -= row["mem"]
+            left[nd]["mem_sw"] -= row["mem_sw"]
+            left[nd]["core"] &= ~row["core"]
+            left[nd]["gres"] &= ~row["gres"]
+            ok_nodes.append(nd)
+            rowsj.append(row)
+        if not ok_nodes:
+            continue
+        r_node += ok_nodes
+        r_res += rowsj
+        r_off.append(len(r_node))
+        r_start.append(NOW - int(rng.integers(1, 5000)))
+        r_end.append(NOW + int(rng.integers(-10, 3 * DAY if rng.random() < 0.7 else 9 * DAY)))
+        r_nn.append(len(ok_nodes))
+        r_cpu.append(sum(int(r["cpu_raw"]) for r in rowsj))
+        r_mem.append(sum(int(r["mem"]) for r in rowsj))
+    k = len(r_start)
+    running = Running(r_start, r_end, r_nn, rng.choice([1000, 2000], k), rng.choice([1000, 5000], k),
+                      rng.integers(0, 6, k), r_cpu, r_mem, r_off, np.array(r_node, np.uint32),
+                      np.array(r_res, RES_IN_NODE) if r_res else np.zeros(0, RES_IN_NODE))
+
+    part = rng.integers(0, n_parts, n_jobs).astype(np.uint32)
+    cap = np.array(usable)[part]
+    node_num = rng.choice([1, 1, 1, 1, 2, 2, 3], n_jobs)
+    w = rng.random(n_jobs) < p_wide
+    node_num[w] = np.minimum(rng.choice(wide, int(w.sum())), cap[w])
+    full = rng.random(n_jobs) < p_full
+    node_num[full] = cap[full]
+    node_num = node_num.astype(np.uint32)
+    big = node_num > 3
+    cores = np.where(big, rng.choice([1, 1, 2, 4, 8], n_jobs), rng.choice([1, 2, 4, 16, 32, 64, 100, 128, 160], n_jobs))
+    cpus_raw = cores * 256
+    fr = rng.random(n_jobs) < 0.1
+    cpus_raw[fr] = rng.choice([64, 128, 384], int(fr.sum()))
+    tpn = np.ones(n_jobs, np.uint32)
+    tpn_max = tpn.copy()
+    gen = (rng.random(n_jobs) < p_general) & (node_num <= 127)
+    tpn[gen] = rng.integers(1, 3, int(gen.sum()))
+    tpn_max[gen] = tpn[gen] + rng.integers(1, 4, int(gen.sum()))
+    ntasks = (node_num * tpn + rng.integers(0, 1 << 30, n_jobs) % (node_num * (tpn_max - tpn) + 1)).astype(np.uint32)
+    cpus_raw = np.where(gen, np.minimum(cpus_raw, 4 * 256), cpus_raw)
+    gt = np.zeros((n_jobs, 8), np.uint16)
+    gs = np.zeros((n_jobs, GRES_ENTRIES), np.uint16)
+    for i in range(n_jobs):
+        if rng.random() < (0.25 if big[i] else 0.5):
+            for e in rng.choice(GRES_ENTRIES, int(rng.integers(1, 3)), replace=False):
+                c = int(rng.choice([1, 1, 2, 3, 4, 8, 16])) if not big[i] else 1
+                if rng.random() < 0.6:
+                    gs[i, e] += c
+                    gt[i, names[e]] += c + (int(rng.integers(0, 2)) if rng.random() < 0.3 else 0)
+                else:
+                    gt[i, names[e]] += c
+    mem_task = rng.integers(1, 9, n_jobs).astype(np.uint64) * GiB // 2
+    mem_node = np.where(rng.random(n_jobs) < 0.2, rng.integers(0, 4, n_jobs), 0).astype(np.uint64) * GiB
+    views = _views(n_jobs, cpus_raw, mem_task, node_num, ntasks, gt, gs, mem_node)
+    mand = np.zeros(n_jobs) if fifo else (rng.permutation(n_jobs) + 1) * 997.0 + 0.5
+    tl = _log_uniform(rng, 60, 3600 if short else 3 * DAY, n_jobs)
+    submit = NOW - 1 - rng.permutation(9 * DAY)[:n_jobs]
+    pend = _pending(n_jobs, part, tl, submit, node_num, ntasks, views,
+                    rng.choice([1000, 2000, 3000], n_jobs).astype(np.uint32),
+                    rng.choice([1000, 2000, 5000], n_jobs).astype(np.uint32),
+                    account=rng.integers(0, 6, n_jobs).astype(np.uint32),
+                    qos=rng.integers(0, 3, n_jobs).astype(np.uint32),
+                    user=rng.integers(0, 20, n_jobs).astype(np.uint32),
+                    exclusive=(rng.random(n_jobs) < 0.03).astype(np.uint8), ntpn=(tpn, tpn_max), mandated=mand)
+    cfg = Config(priority_type=0 if fifo else 1, scheduled_batch_size=limit or n_jobs, cost_policy=cost_policy,
+                 weight_age=500, weight_fair_share=10000, weight_job_size=300,
+                 weight_partition=1000, weight_qos=1_000_000, favor_small=bool(seed & 1))
+    return cfg, cluster, running, pend, NOW
+
+
 def overlap_partitions(case, seed, frac=0.4, which=None):
     """The same case with overlapping partitions: every partition (or only those in
     `which`) also lists a share of the previous partition's nodes, so those nodes have
