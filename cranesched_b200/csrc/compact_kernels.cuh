@@ -6,7 +6,7 @@
 // open entries, on the device, where the gate state lives:
 //   live rows   k_rt_live_keys + the stable LSD radix sort (the regroup's): the live rows
 //               first, in row order; k_cp_map scatters their ranks into the old -> new map
-//   columns     one gather per table (k_cp_pending, k_cp_running): new row c = c-th live row
+//   columns     one gather per table (k_cp_cols, the regroup's too): new row c = c-th live row
 //   CSR tables  lengths of the live rows, their exclusive scan (k_sort_scan) and one warp
 //               per row copying its entries (k_cp_csr)
 //   entries     k_cp_ent_keys flags the open entries of live rows, the same sort lists them
@@ -30,82 +30,43 @@ __global__ void k_cp_map(const uint32_t* live, uint32_t n_live, uint32_t* map) {
   if (c < n_live) map[live[c]] = c;
 }
 
-// The fixed-width columns of the pending table; optional columns are null when the table
-// has none. Gate columns are copied for the new rows [0, gate_n).
-struct PendingCols {
-  uint32_t* partition;
-  int64_t* time_limit;
-  int64_t* submit_time;
-  uint32_t* node_num;
-  uint32_t* ntpn_min;
-  uint32_t* ntpn_max;
-  uint32_t* ntasks;
-  uint8_t* exclusive;
-  uint32_t* partition_priority;
-  uint32_t* qos_priority;
-  uint32_t* account;
-  uint32_t* qos;
-  uint32_t* user;
-  double* mandated;
-  uint32_t* reservation;
-  View* req_node;
-  View* req_task;
-  View* req_total;
-  uint8_t* held;
-  int64_t* begin;
-  uint8_t* is_or;
-  uint32_t* open;
-  long long* ready;
+// One fixed-width column of a gather: new row c takes old row live ? live[c] : c, for the
+// new rows c < rows
+struct ColCopy {
+  const void* src;
+  void* dst;
+  uint32_t bytes;  // of an element
+  uint32_t rows;
 };
 
-__global__ void k_cp_pending(PendingCols s, PendingCols d, const uint32_t* live, uint32_t n_live, uint32_t gate_n) {
-  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= n_live) return;
-  const uint32_t r = live[c];
-  d.partition[c] = s.partition[r];
-  d.time_limit[c] = s.time_limit[r];
-  d.submit_time[c] = s.submit_time[r];
-  d.node_num[c] = s.node_num[r];
-  d.ntpn_min[c] = s.ntpn_min[r];
-  d.ntpn_max[c] = s.ntpn_max[r];
-  d.ntasks[c] = s.ntasks[r];
-  d.exclusive[c] = s.exclusive[r];
-  d.partition_priority[c] = s.partition_priority[r];
-  d.qos_priority[c] = s.qos_priority[r];
-  d.account[c] = s.account[r];
-  if (d.qos) {
-    d.qos[c] = s.qos[r];
-    d.user[c] = s.user[r];
-  }
-  if (d.mandated) d.mandated[c] = s.mandated[r];
-  if (d.reservation) d.reservation[c] = s.reservation[r];
-  d.req_node[c] = s.req_node[r];
-  d.req_task[c] = s.req_task[r];
-  d.req_total[c] = s.req_total[r];
-  if (c < gate_n) {
-    d.held[c] = s.held[r];
-    d.begin[c] = s.begin[r];
-    d.is_or[c] = s.is_or[r];
-    d.open[c] = s.open[r];
-    d.ready[c] = s.ready[r];
-  }
+// The columns of one table (the pending table's 18 with the gate's 5 at most)
+constexpr int kMaxCols = 24;
+struct ColSet {
+  uint32_t n;
+  ColCopy col[kMaxCols];
+};
+
+template <class W>
+__device__ __forceinline__ void cp_elem(const ColCopy& d, uint32_t r, uint32_t c) {
+  const uint32_t w = d.bytes / sizeof(W);
+  const W* s = static_cast<const W*>(d.src) + (size_t)r * w;
+  W* t = static_cast<W*>(d.dst) + (size_t)c * w;
+  for (uint32_t k = 0; k < w; ++k) t[k] = s[k];
 }
 
-// The fixed-width columns of the running table (alloc_off, alloc_node, alloc_res and dead
-// are not read: the CSR goes through k_cp_csr, the new rows are all live)
-__global__ void k_cp_running(RunTableDev s, RunTableDev d, const uint32_t* live, uint32_t n_live) {
+// Thread per new row, every column of the set in turn; elements go in 8-byte words when
+// their size allows (Row and View are 8-byte aligned)
+__global__ void k_cp_cols(ColSet s, const uint32_t* live, uint32_t n_live) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= n_live) return;
-  const uint32_t r = live[c];
-  d.start_time[c] = s.start_time[r];
-  d.end_time[c] = s.end_time[r];
-  d.node_num[c] = s.node_num[r];
-  d.partition_priority[c] = s.partition_priority[r];
-  d.qos_priority[c] = s.qos_priority[r];
-  d.account[c] = s.account[r];
-  d.reservation[c] = s.reservation[r];
-  d.view_cpu_raw[c] = s.view_cpu_raw[r];
-  d.view_mem[c] = s.view_mem[r];
+  const uint32_t r = live ? live[c] : c;
+  for (uint32_t k = 0; k < s.n; ++k) {
+    const ColCopy& d = s.col[k];
+    if (c >= d.rows) continue;
+    if (d.bytes % 8 == 0) cp_elem<uint64_t>(d, r, c);
+    else if (d.bytes % 4 == 0) cp_elem<uint32_t>(d, r, c);
+    else cp_elem<uint8_t>(d, r, c);
+  }
 }
 
 // len[c] = entries of the c-th live row of a CSR table, len[n_live] = 0: the exclusive
@@ -144,9 +105,8 @@ __global__ void k_cp_ent_keys(GateDev g, const uint8_t* pd_dead, uint64_t* keys,
 
 // The kept entries in entry order: dependent through the pending map, dependee through
 // the pending or the running map by kind (an erased dependee becomes kRowNone, which no
-// event row matches); a null map is the identity. `delay` is the new delay column
-// (GateDev's is read-only).
-__global__ void k_cp_entries(GateDev s, GateDev d, uint64_t* delay, const uint32_t* keep, uint32_t n_keep,
+// event row matches); a null map is the identity.
+__global__ void k_cp_entries(GateDev s, GateDev d, const uint32_t* keep, uint32_t n_keep,
                              const uint32_t* pd_map, const uint32_t* rr_map) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= n_keep) return;
@@ -161,7 +121,7 @@ __global__ void k_cp_entries(GateDev s, GateDev d, uint64_t* delay, const uint32
   d.kind[c] = kind;
   d.type[c] = s.type[e];
   d.live[c] = 1;
-  delay[c] = s.delay[e];
+  d.delay[c] = s.delay[e];
 }
 
 }  // namespace crane

@@ -44,7 +44,7 @@ struct GateDev {
   uint8_t* kind;           // kDepPending / kDepRunning
   uint8_t* type;
   uint8_t* live;
-  const uint64_t* delay;
+  uint64_t* delay;
 };
 
 // The events of one call. `rows` are the call's rows sorted ascending, `pos[k]` the

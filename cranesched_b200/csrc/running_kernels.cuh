@@ -35,18 +35,6 @@ struct RunTableDev {
   const uint8_t* dead;      // [n] tombstones
 };
 
-// The dense per-job columns of RunningDev, written by the regroup
-struct RunningCols {
-  int64_t* start_time;
-  int64_t* end_time;
-  uint32_t* node_num;
-  uint32_t* partition_priority;
-  uint32_t* qos_priority;
-  uint32_t* account;
-  int64_t* view_cpu_raw;
-  uint64_t* view_mem;
-};
-
 // What a running job's allocation on a node is looked up in: the node states of the
 // partitions and of the reservations (crane_sched::build_layout)
 struct NodeStateMap {
@@ -127,21 +115,6 @@ __global__ void k_rt_live_keys(const uint8_t* dead, uint32_t n, uint64_t* keys, 
     keys[r] = dead[r] ? 1u : 0u;
     vals[r] = r;
   }
-}
-
-// The dense per-job columns: job c of the view is the c-th live row (live == null: row c)
-__global__ void k_rt_gather(RunTableDev rt, const uint32_t* live, uint32_t n_live, RunningCols o) {
-  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= n_live) return;
-  const uint32_t r = live ? live[c] : c;
-  o.start_time[c] = rt.start_time[r];
-  o.end_time[c] = rt.end_time[r];
-  o.node_num[c] = rt.node_num[r];
-  o.partition_priority[c] = rt.partition_priority[r];
-  o.qos_priority[c] = rt.qos_priority[r];
-  o.account[c] = rt.account[r];
-  o.view_cpu_raw[c] = rt.view_cpu_raw[r];
-  o.view_mem[c] = rt.view_mem[r];
 }
 
 // One warp per row: key of every allocation entry = its node state in bits 0-31 (n_slots

@@ -47,6 +47,11 @@ struct DBuf {
   DBuf() = default;
   DBuf(const DBuf&) = delete;
   DBuf& operator=(const DBuf&) = delete;
+  DBuf(DBuf&& o) noexcept { swap(o); }
+  DBuf& operator=(DBuf&& o) noexcept {
+    swap(o);
+    return *this;
+  }
   ~DBuf() {
     if (p) cudaFree(p);
   }
@@ -85,6 +90,256 @@ struct DBuf {
     if (p) cudaFree(p);
     p = nullptr;
     cap = 0;
+  }
+};
+
+// Each table below lists its fixed-width columns once, in each(o, f), which calls
+// f(column, o's column) for every column the table has: allocation, growth and the
+// gathers of crane_sched_compact and of the regroup go through that list. A table is
+// replaced as a whole (std::swap): compaction builds a fresh one.
+
+// Every fixed-width column of table `t` holds `rows` rows (their contents go)
+template <class Table>
+cudaError_t ensure_cols(Table& t, size_t rows) {
+  cudaError_t e = cudaSuccess;
+  t.each(t, [&](auto& c, auto&) { if (e == cudaSuccess) e = c.ensure(std::max<size_t>(rows, 1)); });
+  return e;
+}
+
+// Every fixed-width column of table `t` grows to `rows` rows, keeping its first `keep`
+template <class Table>
+cudaError_t grow_cols(Table& t, size_t rows, size_t keep, cudaStream_t st) {
+  cudaError_t e = cudaSuccess;
+  t.each(t, [&](auto& c, auto&) { if (e == cudaSuccess) e = c.grow(rows, keep, st); });
+  return e;
+}
+
+// A gather visitor: each column pair (old, new) it is given joins `cs`, for the new rows [0, rows)
+inline auto gather_to(ColSet& cs, uint32_t rows) {
+  return [&cs, rows](const auto& from, auto& to) {
+    if (cs.n < kMaxCols) cs.col[cs.n] = ColCopy{from.p, to.p, (uint32_t)sizeof(*from.p), rows};
+    cs.n++;
+  };
+}
+
+// A resident table's rows keep their index until crane_sched_compact; an erased row
+// stays behind as a tombstone.
+struct Tombstones {
+  uint32_t n = 0;  // rows, tombstones included
+  uint32_t n_dead = 0;
+  std::vector<uint8_t> h_dead;
+  DBuf<uint8_t> d_dead;
+  const uint8_t* dead() const { return n_dead ? d_dead.p : nullptr; }
+  // `rows` rows, all live
+  cudaError_t alloc_live(uint32_t rows, cudaStream_t st) {
+    n = rows;
+    n_dead = 0;
+    h_dead.assign(rows, 0);
+    cudaError_t e = d_dead.ensure(std::max<uint32_t>(rows, 1));
+    return e == cudaSuccess ? cudaMemsetAsync(d_dead.p, 0, std::max<uint32_t>(rows, 1), st) : e;
+  }
+};
+
+// The resident pending table (crane_sched_pending_append)
+struct PendingTable : Tombstones {
+  uint64_t total_alloc = 0;  // allocation rows of a run's placements: the sum of node_num
+  // optional columns, all-or-nothing over the life of the table
+  bool have_qos_cols = false, have_mandated = false, have_pd_resv = false, have_lists_incl = false,
+       have_lists_excl = false;
+  DBuf<uint32_t> d_partition, d_node_num, d_ntpn, d_ntpn_max, d_ntasks, d_part_prio, d_qos_prio, d_account, d_qos,
+      d_user, d_pd_resv;
+  DBuf<int64_t> d_time_limit, d_submit;
+  DBuf<uint8_t> d_exclusive;
+  DBuf<double> d_mandated;
+  DBuf<View> d_req_node, d_req_task, d_req_total;
+  // CSR tables: the rows' allocation slots of a run (the prefix sum of node_num), the node lists
+  DBuf<uint32_t> d_alloc_off, d_incl_off, d_incl_nodes, d_excl_off, d_excl_nodes;
+  // host mirrors
+  std::vector<uint32_t> h_alloc_off = {0}, h_incl_off = {0}, h_excl_off = {0}, h_pd_account;
+
+  template <class F>
+  void each(PendingTable& o, F f) {
+    f(d_partition, o.d_partition);
+    f(d_time_limit, o.d_time_limit);
+    f(d_submit, o.d_submit);
+    f(d_node_num, o.d_node_num);
+    f(d_ntpn, o.d_ntpn);
+    f(d_ntpn_max, o.d_ntpn_max);
+    f(d_ntasks, o.d_ntasks);
+    f(d_exclusive, o.d_exclusive);
+    f(d_part_prio, o.d_part_prio);
+    f(d_qos_prio, o.d_qos_prio);
+    f(d_account, o.d_account);
+    f(d_req_node, o.d_req_node);
+    f(d_req_task, o.d_req_task);
+    f(d_req_total, o.d_req_total);
+    if (have_qos_cols) {
+      f(d_qos, o.d_qos);
+      f(d_user, o.d_user);
+    }
+    if (have_mandated) f(d_mandated, o.d_mandated);
+    if (have_pd_resv) f(d_pd_resv, o.d_pd_resv);
+  }
+
+  void reset() {
+    n = n_dead = 0;
+    total_alloc = 0;
+    h_dead.clear();
+    h_alloc_off.assign(1, 0);
+    h_incl_off.assign(1, 0);
+    h_excl_off.assign(1, 0);
+    h_pd_account.clear();
+  }
+
+  PendingDev dev() const {
+    PendingDev pd{};
+    pd.n = n;
+    pd.partition = d_partition.p;
+    pd.time_limit = d_time_limit.p;
+    pd.submit_time = d_submit.p;
+    pd.node_num = d_node_num.p;
+    pd.ntasks_per_node_min = d_ntpn.p;
+    pd.ntasks_per_node_max = d_ntpn_max.p;
+    pd.ntasks = d_ntasks.p;
+    pd.exclusive = d_exclusive.p;
+    pd.partition_priority = d_part_prio.p;
+    pd.qos_priority = d_qos_prio.p;
+    pd.account = d_account.p;
+    pd.mandated_priority = have_mandated ? d_mandated.p : nullptr;
+    pd.req_node = d_req_node.p;
+    pd.req_task = d_req_task.p;
+    pd.req_total = d_req_total.p;
+    pd.incl_off = have_lists_incl ? d_incl_off.p : nullptr;
+    pd.incl_nodes = d_incl_nodes.p;
+    pd.excl_off = have_lists_excl ? d_excl_off.p : nullptr;
+    pd.excl_nodes = d_excl_nodes.p;
+    pd.alloc_off = d_alloc_off.p;
+    pd.reservation = have_pd_resv ? d_pd_resv.p : nullptr;
+    pd.dead = dead();
+    return pd;
+  }
+};
+
+// The gate state of the pending rows [0, n) (gate_kernels.cuh): off until a gate call
+// after pending_reset
+struct GateRows {
+  bool on = false;
+  uint32_t n = 0;
+  std::vector<uint8_t> h_has_deps;  // [n] the row got its dependency list
+  DBuf<uint8_t> d_g_held, d_g_is_or;
+  DBuf<int64_t> d_g_begin;
+  DBuf<long long> d_g_ready;
+  DBuf<uint32_t> d_g_open;
+
+  template <class F>
+  void each(GateRows& o, F f) {
+    f(d_g_held, o.d_g_held);
+    f(d_g_begin, o.d_g_begin);
+    f(d_g_is_or, o.d_g_is_or);
+    f(d_g_open, o.d_g_open);
+    f(d_g_ready, o.d_g_ready);
+  }
+};
+
+// The dependency entries of the gate, live or retired
+struct DepEntries {
+  uint32_t n = 0;
+  DBuf<uint32_t> d_e_dependent, d_e_dependee;
+  DBuf<uint8_t> d_e_kind, d_e_type, d_e_live;
+  DBuf<uint64_t> d_e_delay;
+
+  template <class F>
+  void each(DepEntries& o, F f) {
+    f(d_e_dependent, o.d_e_dependent);
+    f(d_e_dependee, o.d_e_dependee);
+    f(d_e_kind, o.d_e_kind);
+    f(d_e_type, o.d_e_type);
+    f(d_e_live, o.d_e_live);
+    f(d_e_delay, o.d_e_delay);
+  }
+};
+
+GateDev gate_dev(GateRows& g, DepEntries& e, const uint8_t* pd_dead) {
+  GateDev d{};
+  d.n = g.n;
+  d.dead = pd_dead;
+  d.held = g.d_g_held.p;
+  d.begin = g.d_g_begin.p;
+  d.is_or = g.d_g_is_or.p;
+  d.open = g.d_g_open.p;
+  d.ready = g.d_g_ready.p;
+  d.n_ent = e.n;
+  d.dependent = e.d_e_dependent.p;
+  d.dependee = e.d_e_dependee.p;
+  d.kind = e.d_e_kind.p;
+  d.type = e.d_e_type.p;
+  d.live = e.d_e_live.p;
+  d.delay = e.d_e_delay.p;
+  return d;
+}
+
+// The fixed-width columns of running jobs: the resident table's, and the tick's dense
+// view of its live rows (RunningDev)
+struct RunCols {
+  DBuf<int64_t> d_rr_start, d_rr_end, d_rr_cpu;
+  DBuf<uint32_t> d_rr_node_num, d_rr_part_prio, d_rr_qos_prio, d_rr_account;
+  DBuf<uint64_t> d_rr_mem;
+
+  template <class F>
+  void each(RunCols& o, F f) {
+    f(d_rr_start, o.d_rr_start);
+    f(d_rr_end, o.d_rr_end);
+    f(d_rr_node_num, o.d_rr_node_num);
+    f(d_rr_part_prio, o.d_rr_part_prio);
+    f(d_rr_qos_prio, o.d_rr_qos_prio);
+    f(d_rr_account, o.d_rr_account);
+    f(d_rr_cpu, o.d_rr_cpu);
+    f(d_rr_mem, o.d_rr_mem);
+  }
+};
+
+// The resident running table (crane_sched_running_append, crane_sched_start)
+struct RunningTable : Tombstones, RunCols {
+  uint32_t node_bound = 0;  // every node index of a row is below this
+  bool dirty = true;        // rows or the node-state layout changed since the last regroup
+  DBuf<uint32_t> d_rr_resv;  // not in the dense view: the regroup reads it to group allocations by node state
+  DBuf<uint32_t> d_rr_alloc_off, d_rr_alloc_node;  // CSR over (node, res) entries
+  DBuf<Row> d_rr_alloc_res;
+  // host mirrors
+  std::vector<uint32_t> h_rr_alloc_off = {0}, h_rr_account;
+
+  template <class F>
+  void each(RunningTable& o, F f) {
+    RunCols::each(o, f);
+    f(d_rr_resv, o.d_rr_resv);
+  }
+
+  void reset() {
+    n = n_dead = 0;
+    h_dead.clear();
+    h_rr_alloc_off.assign(1, 0);
+    h_rr_account.clear();
+    node_bound = 0;
+    dirty = true;
+  }
+
+  RunTableDev dev() {
+    RunTableDev rt{};
+    rt.n = n;
+    rt.start_time = d_rr_start.p;
+    rt.end_time = d_rr_end.p;
+    rt.node_num = d_rr_node_num.p;
+    rt.partition_priority = d_rr_part_prio.p;
+    rt.qos_priority = d_rr_qos_prio.p;
+    rt.account = d_rr_account.p;
+    rt.reservation = d_rr_resv.p;
+    rt.view_cpu_raw = d_rr_cpu.p;
+    rt.view_mem = d_rr_mem.p;
+    rt.alloc_off = d_rr_alloc_off.p;
+    rt.alloc_node = d_rr_alloc_node.p;
+    rt.alloc_res = d_rr_alloc_res.p;
+    rt.dead = d_dead.p;
+    return rt;
   }
 };
 
@@ -150,60 +405,25 @@ struct crane_sched {
   DBuf<uint8_t> d_skip;
   DBuf<int64_t> d_first_resv, d_resv_start, d_resv_end;
   DBuf<uint32_t> d_q_off;
-  DBuf<uint32_t> d_slot_resv, d_rsv_off, d_rsv_id, d_vpart, d_pd_resv, d_sched_nparts, d_part_comp, d_part_cidx, d_sched_owner;
+  DBuf<uint32_t> d_slot_resv, d_rsv_off, d_rsv_id, d_vpart, d_sched_nparts, d_part_comp, d_part_cidx, d_sched_owner;
   DBuf<uint8_t> d_slot_memb;
   DBuf<Row> d_rsv_res;
-  bool have_pd_resv = false;
 
-  // pending (device)
-  uint32_t n_pending = 0, n_running = 0, n_accounts = 0;
-  uint64_t total_alloc = 0;
-  bool have_lists_incl = false, have_lists_excl = false, have_mandated = false;
-  std::vector<uint32_t> h_alloc_off;
-  // device-resident pending table: host mirrors of the small columns, tombstones
-  std::vector<uint32_t> h_pd_account, h_incl_off, h_excl_off;
-  std::vector<uint8_t> h_dead;
-  uint32_t n_dead = 0;
-  DBuf<uint8_t> d_dead;
-  DBuf<uint32_t> d_erase_rows;
-  DBuf<uint32_t> d_ntpn_max, d_ntasks;
-  DBuf<uint32_t> d_partition, d_node_num, d_ntpn, d_part_prio, d_qos_prio, d_account, d_alloc_off;
-  DBuf<int64_t> d_time_limit, d_submit;
-  DBuf<uint8_t> d_exclusive;
-  DBuf<double> d_mandated;
-  DBuf<View> d_req_node, d_req_task, d_req_total;
-  DBuf<uint32_t> d_incl_off, d_incl_nodes, d_excl_off, d_excl_nodes;
-  // device-resident running table: rows keep their index until the table is replaced,
-  // an erased row is a tombstone; host mirrors of the small columns
-  uint32_t n_rr = 0, n_rr_dead = 0;
-  std::vector<uint32_t> h_rr_alloc_off = {0}, h_rr_account;
-  std::vector<uint8_t> h_rr_dead;
-  uint32_t rr_node_bound = 0;  // every node index of a row is below this
-  bool rr_dirty = true;        // rows or the node-state layout changed since the last regroup
-  DBuf<int64_t> d_rr_start, d_rr_end, d_rr_cpu;
-  DBuf<uint32_t> d_rr_node_num, d_rr_part_prio, d_rr_qos_prio, d_rr_account, d_rr_resv, d_rr_alloc_off, d_rr_alloc_node;
-  DBuf<uint64_t> d_rr_mem;
-  DBuf<Row> d_rr_alloc_res;
-  DBuf<uint8_t> d_rr_dead;
-  DBuf<uint32_t> d_r_node_off, d_r_node, d_flag, d_start_rows;
+  // the resident tables
+  PendingTable pd;
+  GateRows gate;
+  DepEntries ent;
+  RunningTable rr;
+  uint32_t n_running = 0, n_accounts = 0;  // the tick's live running rows, accounts
+  DBuf<uint32_t> d_erase_rows, d_r_node_off, d_r_node, d_flag, d_start_rows;
   // the tick's view of the live rows (RunningDev), built by the regroup
-  DBuf<int64_t> d_rn_start, d_rn_end, d_rn_cpu, d_rn_slot_end;
-  DBuf<uint32_t> d_rn_node_num, d_rn_part_prio, d_rn_qos_prio, d_rn_account, d_rn_slot_off, d_rn_acc_off, d_rn_acc_job;
-  DBuf<uint64_t> d_rn_mem, d_rn_acc_key;
+  RunCols rn;
+  DBuf<int64_t> d_rn_slot_end;
+  DBuf<uint32_t> d_rn_slot_off, d_rn_acc_off, d_rn_acc_job;
+  DBuf<uint64_t> d_rn_acc_key;
   DBuf<Row> d_rn_slot_res;
   DBuf<uint8_t> d_acc_present;
-  // the gate of the pending table (gate_kernels.cuh): off until a gate call after pending_reset
-  bool gate_on = false;
-  uint32_t gate_n = 0;              // rows [0, gate_n) have gate state
-  std::vector<uint8_t> h_has_deps;  // [gate_n] the row got its dependency list
-  uint32_t n_ent = 0;               // dependency entries, live or retired
-  DBuf<uint8_t> d_g_held, d_g_is_or, d_g_code;
-  DBuf<int64_t> d_g_begin;
-  DBuf<long long> d_g_ready;
-  DBuf<uint32_t> d_g_open;
-  DBuf<uint32_t> d_e_dependent, d_e_dependee;
-  DBuf<uint8_t> d_e_kind, d_e_type, d_e_live;
-  DBuf<uint64_t> d_e_delay;
+  DBuf<uint8_t> d_g_code;  // the run's exclusion code of every pending row (k_gate)
   DBuf<uint32_t> d_ev_rows, d_ev_u32;  // per call: sorted rows + their positions | exit codes, offsets
   DBuf<int64_t> d_ev_i64;              // per call: end / event times, begin times
   DBuf<uint8_t> d_ev_u8;               // per call: held, is_or
@@ -227,8 +447,7 @@ struct crane_sched {
   std::vector<uint32_t> h_part_owner, h_part_list;
   DBuf<uint32_t> d_part_owner, d_part_list;
   // QoS post-filter (R12)
-  bool have_qos_cols = false;
-  DBuf<uint32_t> d_qos, d_user, d_q_u32, d_q_chain_off, d_q_chain;
+  DBuf<uint32_t> d_q_u32, d_q_chain_off, d_q_chain;
   DBuf<int64_t> d_q_i64;
   DBuf<uint8_t> d_q_valid;
   DBuf<crane_tres_limit_t> d_q_tres;
@@ -400,64 +619,16 @@ int radix_sort(crane_sched* h, uint32_t n, int nbits, uint64_t** keys, uint32_t*
   return CRANE_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-const char* crane_sched_last_error(const crane_sched_t* h) { return h ? h->err.c_str() : "null handle"; }
-
-int crane_sched_create(const crane_sched_config_t* cfg, int device, crane_sched_t** out) {
-  if (!cfg || !out) return CRANE_EINVAL;
-  *out = nullptr;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return CRANE_ENODEV;
-  if (cfg->max_jobs_per_node < 2 || cfg->max_jobs_per_node > 65000) return CRANE_EINVAL;
-  if (cfg->cost_policy > 1) return CRANE_ENOSYS;  // 0 MinCpuTimeRatioFirst (JobScheduler.h:40), 1 BestFit (ours, config 4)
-  if (device >= 64) return CRANE_EINVAL;
-  int slot = -1;
-  {
-    std::lock_guard<std::mutex> lk(g_slot_mu);
-    for (int k = 0; k < kDictSlots; ++k)
-      if (!(g_slots_used[device] >> k & 1u)) { slot = k; g_slots_used[device] |= 1u << k; break; }
-  }
-  if (slot < 0) return CRANE_ENOSYS;  // more than kDictSlots live handles on one device
-  crane_sched* h = new crane_sched();
-  h->cfg = *cfg;
-  h->device = device;
-  h->dict_slot = slot;
-  if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
-    delete h;
-    return CRANE_ENODEV;
-  }
-  for (auto& e : h->ev) cudaEventCreate(&e);
-  int n_sm = 0, smem_optin = 0;
-  if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device) != cudaSuccess ||
-      cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess || n_sm <= 0) {
-    delete h;
-    return CRANE_ENODEV;
-  }
-  h->n_sm = (uint32_t)n_sm;
-  {
-    // k_commit2: everything a block may opt in to (227 KB on H100) beyond the kernel's static tables
-    size_t stat = 20 * 1024;
-#ifndef CRANE_EMU
-    cudaFuncAttributes fa;
-    if (cudaFuncGetAttributes(&fa, k_commit2) == cudaSuccess) stat = fa.sharedSizeBytes;
-#endif
-    const size_t sm_total = (size_t)smem_optin;
-    h->v2_budget = sm_total > stat + 1024 ? sm_total - stat - 1024 : 0;
-    cudaFuncSetAttribute(k_commit2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->v2_budget);
-  }
-  h->tl_cap = cfg->max_jobs_per_node + 1;
-  *out = h;
+// k_cp_cols over the new rows [0, n)
+int gather(crane_sched* h, const ColSet& cs, const uint32_t* live, uint32_t n) {
+  if (cs.n > kMaxCols) return fail(h, CRANE_ECUDA, "gather: %u columns, more than %d", cs.n, kMaxCols);
+  if (n) CRANE_LAUNCH(k_cp_cols, (n + 255) / 256, 256, 0, h->stream, cs, live, n);
   return CRANE_OK;
 }
 
-void crane_sched_destroy(crane_sched_t* h) { delete h; }
-
 // Slot layout of the node states: the usable nodes of every partition (contiguous per
 // partition), then the nodes of every reservation; device copies of the cluster tables.
-static int build_layout(crane_sched* h) {
+int build_layout(crane_sched* h) {
   h->h_node_slot.assign(h->n_nodes, 0xffffffffu);
   h->h_slot_node.clear();
   std::vector<Row> slot_total;
@@ -617,12 +788,598 @@ static int build_layout(crane_sched* h) {
   CU(h->d_part_job_off.ensure(h->n_vparts + 2));
   CU(cudaStreamSynchronize(h->stream));
   h->stage = kCluster;
-  h->rr_dirty = true;  // the running view is grouped by node state
+  h->rr.dirty = true;  // the running view is grouped by node state
   h->shard_rank = 0;
   h->shard_n = 1;  // a new cluster: the partition -> rank table has to be set again
   return CRANE_OK;
 }
 
+template <class T>
+int h2d_at(crane_sched* h, DBuf<T>& dst, const T* src, size_t base, size_t n) {
+  CU(dst.grow(std::max<size_t>(base + n, 1), base, h->stream));
+  if (n) CU(cudaMemcpyAsync(dst.p + base, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream));
+  return CRANE_OK;
+}
+#define H2D_AT(buf, src, base, n) TRY(h2d_at(h, buf, src, (size_t)(base), (size_t)(n)))
+
+// Appends the rows of `pd` to the device-resident pending table (rows keep job-id
+// order: the reference's pending map is a btree over job ids, JobScheduler.cpp:1092).
+int pending_append(crane_sched* h, const crane_pending_t* pd) {
+  const uint32_t base = h->pd.n, N = pd->n;
+  if (N && (!pd->partition || !pd->time_limit || !pd->submit_time || !pd->node_num || !pd->ntasks ||
+            !pd->ntasks_per_node_min || !pd->ntasks_per_node_max || !pd->exclusive || !pd->partition_priority ||
+            !pd->qos_priority || !pd->account || !pd->req_node || !pd->req_task || !pd->req_total))
+    return fail(h, CRANE_EINVAL, "pending: null column");
+  if ((uint64_t)base + N > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "pending: too many rows");
+  // optional columns are all-or-nothing over the life of the table
+  if (base) {
+    if ((pd->qos != nullptr && pd->user != nullptr) != h->pd.have_qos_cols || (pd->mandated_priority != nullptr) != h->pd.have_mandated ||
+        (pd->reservation != nullptr) != h->pd.have_pd_resv || (pd->incl_off != nullptr) != h->pd.have_lists_incl ||
+        (pd->excl_off != nullptr) != h->pd.have_lists_excl)
+      return fail(h, CRANE_EINVAL, "pending_append: optional columns (qos/user, mandated_priority, reservation, node lists) must match the table's");
+  } else {
+    h->pd.reset();
+    h->pd.have_qos_cols = pd->qos != nullptr && pd->user != nullptr;
+    h->pd.have_mandated = pd->mandated_priority != nullptr;
+    h->pd.have_pd_resv = pd->reservation != nullptr;
+    h->pd.have_lists_incl = pd->incl_off != nullptr;
+    h->pd.have_lists_excl = pd->excl_off != nullptr;
+  }
+  // ---- validation + alloc_off (prefix sum of node_num over all rows) -----------
+  uint64_t acc = h->pd.h_alloc_off.back();
+  for (uint32_t i = 0; i < N; ++i) {
+    if (pd->node_num[i] == 0) return fail(h, CRANE_EINVAL, "pending[%u]: node_num == 0", i);
+    if (pd->time_limit[i] < 1) return fail(h, CRANE_EINVAL, "pending[%u]: time_limit < 1", i);
+    const uint32_t t = pd->ntasks_per_node_min[i], tmax = pd->ntasks_per_node_max[i];
+    if (t == 0 || tmax < t) return fail(h, CRANE_EINVAL, "pending[%u]: ntasks_per_node_min/max", i);
+    // general task distribution (the top-K heaps of JobScheduler.cpp:5193-5205): heaps of up to 127 nodes
+    if ((tmax != t || (uint64_t)t * pd->node_num[i] != pd->ntasks[i]) && pd->node_num[i] >= (uint32_t)kHeapMax)
+      return fail(h, CRANE_ENOSYS, "pending[%u]: a job with a ntasks_per_node range wider than %d nodes", i, kHeapMax - 1);
+    if ((uint64_t)tmax * pd->node_num[i] < pd->ntasks[i] || (uint64_t)t * pd->node_num[i] > pd->ntasks[i])
+      return fail(h, CRANE_EINVAL, "pending[%u]: ntasks outside [node_num*ntpn_min, node_num*ntpn_max]", i);
+    if (pd->req_node[i].cpu_raw < 0 || pd->req_task[i].cpu_raw < 0)
+      return fail(h, CRANE_EINVAL, "pending[%u]: negative cpu request", i);
+    if (pd->account[i] > (1u << 24)) return fail(h, CRANE_EINVAL, "account ids must be dense (< 2^24)");
+    acc += pd->node_num[i];
+    if (acc > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "pending: sum(node_num) overflows");
+  }
+  if (pd->incl_off) TRY(check_node_list(h, "pending: include list", pd->incl_off, pd->incl_nodes, N));
+  if (pd->excl_off) TRY(check_node_list(h, "pending: exclude list", pd->excl_off, pd->excl_nodes, N));
+  // ---- columns ----------------------------------------------------------------
+  H2D_AT(h->pd.d_partition, pd->partition, base, N);
+  H2D_AT(h->pd.d_time_limit, pd->time_limit, base, N);
+  H2D_AT(h->pd.d_submit, pd->submit_time, base, N);
+  H2D_AT(h->pd.d_node_num, pd->node_num, base, N);
+  H2D_AT(h->pd.d_ntpn, pd->ntasks_per_node_min, base, N);
+  H2D_AT(h->pd.d_ntpn_max, pd->ntasks_per_node_max, base, N);
+  H2D_AT(h->pd.d_ntasks, pd->ntasks, base, N);
+  H2D_AT(h->pd.d_exclusive, pd->exclusive, base, N);
+  H2D_AT(h->pd.d_part_prio, pd->partition_priority, base, N);
+  H2D_AT(h->pd.d_qos_prio, pd->qos_priority, base, N);
+  H2D_AT(h->pd.d_account, pd->account, base, N);
+  if (h->pd.have_qos_cols) {
+    H2D_AT(h->pd.d_qos, pd->qos, base, N);
+    H2D_AT(h->pd.d_user, pd->user, base, N);
+  }
+  if (h->pd.have_mandated) H2D_AT(h->pd.d_mandated, pd->mandated_priority, base, N);
+  H2D_AT(h->pd.d_req_node, reinterpret_cast<const View*>(pd->req_node), base, N);
+  H2D_AT(h->pd.d_req_task, reinterpret_cast<const View*>(pd->req_task), base, N);
+  H2D_AT(h->pd.d_req_total, reinterpret_cast<const View*>(pd->req_total), base, N);
+  if (h->pd.have_pd_resv) H2D_AT(h->pd.d_pd_resv, pd->reservation, base, N);
+  {
+    std::vector<uint8_t> zeros(N, 0);
+    H2D_AT(h->pd.d_dead, zeros.data(), base, N);
+    CU(cudaStreamSynchronize(h->stream));
+  }
+  // host mirrors
+  for (uint32_t i = 0; i < N; ++i) {
+    h->pd.h_alloc_off.push_back(h->pd.h_alloc_off.back() + pd->node_num[i]);
+    h->pd.h_pd_account.push_back(pd->account[i]);
+    h->pd.h_dead.push_back(0);
+  }
+  H2D_AT(h->pd.d_alloc_off, h->pd.h_alloc_off.data() + base, base, (size_t)N + 1);
+  if (h->pd.have_lists_incl) {
+    const uint32_t nb = h->pd.h_incl_off.back();
+    for (uint32_t i = 0; i < N; ++i) h->pd.h_incl_off.push_back(nb + pd->incl_off[i + 1]);
+    H2D_AT(h->pd.d_incl_off, h->pd.h_incl_off.data() + base, base, (size_t)N + 1);
+    H2D_AT(h->pd.d_incl_nodes, pd->incl_nodes, nb, pd->incl_off[N]);
+  }
+  if (h->pd.have_lists_excl) {
+    const uint32_t nb = h->pd.h_excl_off.back();
+    for (uint32_t i = 0; i < N; ++i) h->pd.h_excl_off.push_back(nb + pd->excl_off[i + 1]);
+    H2D_AT(h->pd.d_excl_off, h->pd.h_excl_off.data() + base, base, (size_t)N + 1);
+    H2D_AT(h->pd.d_excl_nodes, pd->excl_nodes, nb, pd->excl_off[N]);
+  }
+  CU(cudaStreamSynchronize(h->stream));
+  h->pd.n = base + N;
+  h->pd.total_alloc = h->pd.h_alloc_off.back();
+  return CRANE_OK;
+}
+
+// The rows of a host running table: the checks of crane_sched_running_append (`replace`:
+// the rows will replace the table rather than extend it)
+int running_check(crane_sched* h, const crane_running_t* rn, bool replace) {
+  const uint32_t R = rn ? rn->n : 0;
+  if (!R) return CRANE_OK;
+  if (!rn->start_time || !rn->end_time || !rn->node_num || !rn->partition_priority || !rn->qos_priority ||
+      !rn->account || !rn->view_cpu_raw || !rn->view_mem)
+    return fail(h, CRANE_EINVAL, "running: null column");
+  TRY(check_offsets(h, "running: alloc_off", rn->alloc_off, R));
+  const uint32_t E = rn->alloc_off[R];
+  if (E && (!rn->alloc_node || !rn->alloc_res)) return fail(h, CRANE_EINVAL, "running: null allocation table");
+  const uint64_t rows = replace ? 0 : h->rr.n, entries = replace ? 0 : h->rr.h_rr_alloc_off.back();
+  if (rows + R > 0xfffffff0ull || entries + E > 0xfffffff0ull)
+    return fail(h, CRANE_EINVAL, "running: too many rows");
+  for (uint32_t j = 0; j < R; ++j) {
+    if (rn->account[j] > (1u << 24)) return fail(h, CRANE_EINVAL, "account ids must be dense (< 2^24)");
+    for (uint32_t k = rn->alloc_off[j]; k < rn->alloc_off[j + 1]; ++k)
+      if (rn->alloc_node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "running[%u]: node out of range", j);
+  }
+  return CRANE_OK;
+}
+
+// Appends the rows of a checked host running table to the resident table
+int running_append(crane_sched* h, const crane_running_t* rn) {
+  const uint32_t base = h->rr.n, R = rn ? rn->n : 0;
+  if (!R) return CRANE_OK;
+  const uint32_t eb = h->rr.h_rr_alloc_off.back(), E = rn->alloc_off[R];
+  H2D_AT(h->rr.d_rr_start, rn->start_time, base, R);
+  H2D_AT(h->rr.d_rr_end, rn->end_time, base, R);
+  H2D_AT(h->rr.d_rr_node_num, rn->node_num, base, R);
+  H2D_AT(h->rr.d_rr_part_prio, rn->partition_priority, base, R);
+  H2D_AT(h->rr.d_rr_qos_prio, rn->qos_priority, base, R);
+  H2D_AT(h->rr.d_rr_account, rn->account, base, R);
+  H2D_AT(h->rr.d_rr_cpu, rn->view_cpu_raw, base, R);
+  H2D_AT(h->rr.d_rr_mem, rn->view_mem, base, R);
+  std::vector<uint32_t> no_resv(rn->reservation ? 0 : R, 0xffffffffu);
+  H2D_AT(h->rr.d_rr_resv, rn->reservation ? rn->reservation : no_resv.data(), base, R);
+  std::vector<uint8_t> zeros(R, 0);
+  H2D_AT(h->rr.d_dead, zeros.data(), base, R);
+  for (uint32_t j = 0; j < R; ++j) {
+    h->rr.h_rr_alloc_off.push_back(eb + rn->alloc_off[j + 1]);
+    h->rr.h_rr_account.push_back(rn->account[j]);
+    h->rr.h_dead.push_back(0);
+  }
+  H2D_AT(h->rr.d_rr_alloc_off, h->rr.h_rr_alloc_off.data() + base, base, (size_t)R + 1);
+  H2D_AT(h->rr.d_rr_alloc_node, rn->alloc_node, eb, E);
+  H2D_AT(h->rr.d_rr_alloc_res, reinterpret_cast<const Row*>(rn->alloc_res), eb, E);
+  for (uint32_t k = 0; k < E; ++k) h->rr.node_bound = std::max(h->rr.node_bound, rn->alloc_node[k] + 1);
+  CU(cudaStreamSynchronize(h->stream));  // (the staging vectors are pageable)
+  h->rr.n = base + R;
+  h->rr.dirty = true;
+  return CRANE_OK;
+}
+
+// The tick's RunningDev view of the live rows, on the device: the dense per-job columns
+// (live rows in row order), the allocations grouped by node state and the jobs grouped by
+// account, both stable (order inside a node state / account is row order, deviation D6).
+int regroup(crane_sched* h, uint32_t R, uint32_t max_rn_account) {
+  cudaStream_t st = h->stream;
+  const uint32_t Rt = h->rr.n, E = h->rr.h_rr_alloc_off.back();
+  const RunTableDev rt = h->rr.dev();
+  CU(ensure_cols(h->rn, R));
+  CU(h->d_rn_acc_key.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_acc_job.ensure(std::max<uint32_t>(R, 1)));
+  CU(h->d_rn_slot_off.ensure((size_t)h->n_slots + 1));
+  CU(h->d_rn_slot_end.ensure(std::max<uint32_t>(E, 1)));
+  CU(h->d_rn_slot_res.ensure(std::max<uint32_t>(E, 1)));
+  CU(h->d_flag.ensure(1));
+  CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
+  uint64_t* keys;
+  uint32_t* vals;
+  // live rows in row order -> the dense columns (without tombstones: every row, in order)
+  if (R) {
+    vals = nullptr;
+    if (h->rr.n_dead) {
+      CRANE_LAUNCH(k_rt_live_keys, (Rt + 255) / 256, 256, 0, st, rt.dead, Rt, h->d_keys_a.p, h->d_vals_a.p);
+      TRY(radix_sort(h, Rt, 8, &keys, &vals));
+    }
+    ColSet cs{};
+    h->rr.RunCols::each(h->rn, gather_to(cs, R));
+    TRY(gather(h, cs, vals, R));
+  }
+  // allocations by node state: stable sort of the entries (row order) by slot
+  if (E) {
+    NodeStateMap m{h->n_nodes, h->n_slots, h->n_comp, h->n_resv, h->d_node_slot.p, h->d_part_base.p, h->d_r_node_off.p, h->d_r_node.p};
+    const uint32_t nb = std::min<uint32_t>((Rt + 7) / 8, 8 * h->n_sm);
+    CRANE_LAUNCH(k_rt_entry_keys, nb, 256, 0, st, rt, m, h->d_keys_a.p, h->d_vals_a.p, h->d_flag.p);
+    int bits = 8;
+    while ((1ull << bits) <= (uint64_t)h->n_slots) bits += 8;
+    TRY(radix_sort(h, E, bits, &keys, &vals));
+    CRANE_LAUNCH(k_rt_offsets, (h->n_slots + 1 + 255) / 256, 256, 0, st, keys, E, h->n_slots, h->d_rn_slot_off.p);
+    CRANE_LAUNCH(k_rt_slot_gather, (E + 255) / 256, 256, 0, st, rt, keys, vals, E, h->d_rn_slot_off.p + h->n_slots,
+                 h->d_rn_slot_end.p, h->d_rn_slot_res.p);
+  } else {
+    CU(cudaMemsetAsync(h->d_rn_slot_off.p, 0, sizeof(uint32_t) * ((size_t)h->n_slots + 1), st));
+  }
+  // jobs by account: stable sort of the view's jobs by account
+  if (R) {
+    CRANE_LAUNCH(k_rt_acc_keys, (R + 255) / 256, 256, 0, st, h->rn.d_rr_account.p, R, h->d_keys_a.p, h->d_vals_a.p);
+    int bits = 8;
+    while ((1ull << bits) <= (uint64_t)max_rn_account) bits += 8;
+    TRY(radix_sort(h, R, bits, &keys, &vals));
+    CU(cudaMemcpyAsync(h->d_rn_acc_key.p, keys, sizeof(uint64_t) * R, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(h->d_rn_acc_job.p, vals, sizeof(uint32_t) * R, cudaMemcpyDeviceToDevice, st));
+  }
+  CU(cudaGetLastError());
+  // a cluster with fewer nodes than the rows name: one flag read back
+  if (E && h->rr.node_bound > h->n_nodes) {
+    uint32_t bad = 0;
+    CU(cudaMemcpyAsync(&bad, h->d_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (bad) return fail(h, CRANE_EINVAL, "running: node out of range");
+  }
+  h->rr.dirty = false;
+  return CRANE_OK;
+}
+
+// "The next run uses the running table as it stands on the device": the view of the
+// live rows (regrouped when the rows or the node-state layout changed) and the work and
+// output buffers for the resident pending table.
+int keep_running(crane_sched* h) {
+  cudaStream_t st = h->stream;
+  const uint32_t N = h->pd.n, Rt = h->rr.n, R = Rt - h->rr.n_dead;
+  const uint32_t E = h->rr.h_rr_alloc_off.back();
+  uint32_t max_rn_account = 0, max_account = 0;
+  for (uint32_t r = 0; r < Rt; ++r)
+    if (!h->rr.h_dead[r]) max_rn_account = std::max(max_rn_account, h->rr.h_rr_account[r]);
+  for (uint32_t i = 0; i < N; ++i) max_account = std::max(max_account, h->pd.h_pd_account[i]);
+  max_account = std::max(max_account, max_rn_account);
+  const uint32_t A = (N + R) ? max_account + 1 : 0;
+
+  // ---- work + output buffers (the sorts of the regroup use the priority sort's) ----
+  size_t n1 = std::max<uint32_t>(N, 1);
+  const size_t ns = std::max<size_t>({n1, (size_t)Rt, (size_t)E});
+  CU(h->d_bounds.ensure(1));
+  CU(h->d_acc_service.ensure(std::max<uint32_t>(A, 1)));
+  CU(h->d_prio.ensure(n1));
+  CU(h->d_keys_a.ensure(ns));
+  CU(h->d_keys_b.ensure(ns));
+  CU(h->d_vals_a.ensure(ns));
+  CU(h->d_vals_b.ensure(ns));
+  uint32_t nq = std::min<uint32_t>(N, h->cfg.scheduled_batch_size);
+  CU(h->d_jobq.ensure(std::max<uint32_t>(nq, 1)));
+  CU(h->d_bitmap.ensure((size_t)std::max<uint32_t>(nq, 1) * h->words_per_row));
+  CU(h->d_reason.ensure(n1));
+  CU(h->d_out_prio.ensure(n1));
+  CU(h->d_out_start.ensure(n1));
+  CU(h->d_out_end.ensure(n1));
+  CU(h->d_out_nalloc.ensure(n1));
+  size_t ta = std::max<uint64_t>(h->pd.total_alloc, 1);
+  CU(h->d_out_node.ensure(ta));
+  CU(h->d_out_ntasks.ensure(ta));
+  CU(h->d_out_res.ensure(ta));
+
+  CU(cudaEventRecord(h->ev[kEvKeepBegin], st));
+  if (h->rr.dirty) TRY(regroup(h, R, max_rn_account));
+  // ---- accounts: offsets of the account groups, accounts present (pending included) ----
+  CU(h->d_rn_acc_off.ensure((size_t)A + 1));
+  CU(h->d_acc_present.ensure(std::max<uint32_t>(A, 1)));
+  CRANE_LAUNCH(k_rt_offsets, (A + 1 + 255) / 256, 256, 0, st, h->d_rn_acc_key.p, R, A, h->d_rn_acc_off.p);
+  CU(cudaMemsetAsync(h->d_acc_present.p, 0, std::max<uint32_t>(A, 1), st));
+  if (N + R)
+    CRANE_LAUNCH(k_acc_present, (N + R + 255) / 256, 256, 0, st, h->pd.d_account.p, h->pd.n_dead ? h->pd.d_dead.p : nullptr, N,
+                 h->rn.d_rr_account.p, R, h->d_acc_present.p);
+  CU(cudaEventRecord(h->ev[kEvKeepEnd], st));
+  CU(cudaGetLastError());
+  h->n_running = R;
+  h->n_accounts = A;
+  return CRANE_OK;
+}
+
+// The running table of this tick from a host table: reset + append + keep_running
+int set_running(crane_sched* h, const crane_running_t* rn) {
+  TRY(running_check(h, rn, true));
+  h->rr.reset();
+  TRY(running_append(h, rn));
+  return keep_running(h);
+}
+
+GateDev gate_dev(crane_sched* h) { return gate_dev(h->gate, h->ent, h->pd.dead()); }
+
+// Turns the gate on and gives the rows appended since the last gate call their state:
+// not held, beginning at InfinitePast, no dependencies
+int gate_fit(crane_sched* h) {
+  h->gate.on = true;
+  const uint32_t from = h->gate.n, to = h->pd.n;
+  if (to <= from) return CRANE_OK;
+  cudaStream_t st = h->stream;
+  CU(grow_cols(h->gate, to, from, st));
+  h->gate.n = to;
+  h->gate.h_has_deps.resize(to, 0);
+  CRANE_LAUNCH(k_gate_init, (to - from + 255) / 256, 256, 0, st, gate_dev(h), from, to);
+  CU(cudaGetLastError());
+  return CRANE_OK;
+}
+
+// The rows of an erase / start / read call: in [0, n_rows), not erased, none listed twice
+template <class Erased>
+int check_rows(crane_sched* h, const char* call, const uint32_t* rows, uint32_t n, uint32_t n_rows, Erased erased) {
+  if (n && !rows) return fail(h, CRANE_EINVAL, "%s: null rows", call);
+  std::vector<uint32_t> sorted(rows, rows + n);
+  std::sort(sorted.begin(), sorted.end());
+  for (uint32_t k = 0; k < n; ++k) {
+    if (sorted[k] >= n_rows) return fail(h, CRANE_EINVAL, "%s: row %u out of range", call, sorted[k]);
+    if (erased(sorted[k])) return fail(h, CRANE_EINVAL, "%s: row %u was erased", call, sorted[k]);
+    if (k && sorted[k] == sorted[k - 1]) return fail(h, CRANE_EINVAL, "%s: row %u listed twice", call, sorted[k]);
+  }
+  return CRANE_OK;
+}
+
+// Erases rows of a table: rows out of range fail, rows already erased and rows listed twice do not
+int erase_rows(crane_sched* h, const char* call, Tombstones& t, const uint32_t* rows, uint32_t n) {
+  if (n && !rows) return CRANE_EINVAL;
+  CU(cudaSetDevice(h->device));
+  for (uint32_t k = 0; k < n; ++k)
+    if (rows[k] >= t.n) return fail(h, CRANE_EINVAL, "%s: row %u out of range", call, rows[k]);
+  lower_stage(h, kCluster);
+  if (!n) return CRANE_OK;
+  for (uint32_t k = 0; k < n; ++k)
+    if (!t.h_dead[rows[k]]) { t.h_dead[rows[k]] = 1; t.n_dead++; }
+  H2D(h->d_erase_rows, rows, n);
+  CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, h->stream, h->d_erase_rows.p, n, t.d_dead.p);
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(h->stream));
+  return CRANE_OK;
+}
+
+// The rows of a call on the device, sorted, followed by their places in the call's list
+int upload_call_rows(crane_sched* h, const uint32_t* rows, uint32_t n) {
+  std::vector<uint32_t> idx(n), buf(2 * (size_t)n);
+  for (uint32_t k = 0; k < n; ++k) idx[k] = k;
+  std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return rows[a] < rows[b]; });
+  for (uint32_t k = 0; k < n; ++k) {
+    buf[k] = rows[idx[k]];
+    buf[n + k] = idx[k];
+  }
+  H2D(h->d_ev_rows, buf.data(), buf.size());
+  CU(cudaStreamSynchronize(h->stream));  // (buf is pageable)
+  return CRANE_OK;
+}
+
+// k_dep_fire over `threads` entries for the events of the call whose rows upload_call_rows placed
+int dep_fire(crane_sched* h, DepEvents ev, uint32_t n_rows, uint32_t threads) {
+  if (!threads) return CRANE_OK;
+  ev.n = n_rows;
+  ev.rows = h->d_ev_rows.p;
+  ev.pos = h->d_ev_rows.p + n_rows;
+  CRANE_LAUNCH(k_dep_fire, (threads + 255) / 256, 256, 0, h->stream, gate_dev(h), ev);
+  CU(cudaGetLastError());
+  return CRANE_OK;
+}
+
+// The live rows of a table of n rows, in row order (the stable sort by tombstone flag),
+// into live[0, n_live), and the old -> new map into map[0, n)
+int live_rows(crane_sched* h, const uint8_t* dead, uint32_t n, uint32_t n_live, uint32_t* live, uint32_t* map) {
+  cudaStream_t st = h->stream;
+  uint64_t* keys;
+  uint32_t* vals;
+  CRANE_LAUNCH(k_rt_live_keys, (n + 255) / 256, 256, 0, st, dead, n, h->d_keys_a.p, h->d_vals_a.p);
+  TRY(radix_sort(h, n, 8, &keys, &vals));
+  if (n_live) CU(cudaMemcpyAsync(live, vals, sizeof(uint32_t) * n_live, cudaMemcpyDeviceToDevice, st));
+  CU(cudaMemsetAsync(map, 0xff, sizeof(uint32_t) * n, st));
+  if (n_live) CRANE_LAUNCH(k_cp_map, (n_live + 255) / 256, 256, 0, st, live, n_live, map);
+  return CRANE_OK;
+}
+
+// new_off[0, n_live] = the offsets of the live rows of a CSR table
+int csr_offsets(crane_sched* h, const uint32_t* off, const uint32_t* live, uint32_t n_live, uint32_t* new_off) {
+  CRANE_LAUNCH(k_cp_lengths, (n_live + 1 + 255) / 256, 256, 0, h->stream, off, live, n_live, new_off);
+  CRANE_LAUNCH(k_sort_scan, 1, 1024, 0, h->stream, new_off, n_live + 1);
+  return CRANE_OK;
+}
+
+// The entries of the live rows of a CSR table at their new offsets
+template <class T>
+int csr_copy(crane_sched* h, const uint32_t* off, const T* src, const uint32_t* live, uint32_t n_live,
+             const uint32_t* new_off, T* dst) {
+  if (!n_live) return CRANE_OK;
+  const uint32_t nb = std::min<uint32_t>((n_live + 7) / 8, 8 * h->n_sm);
+  CRANE_LAUNCH(k_cp_csr<T>, nb, 256, 0, h->stream, off, src, live, n_live, new_off, dst);
+  return CRANE_OK;
+}
+
+// Host mirror of a CSR table's offsets for its live rows
+std::vector<uint32_t> live_offsets(const std::vector<uint32_t>& off, const std::vector<uint8_t>& dead) {
+  std::vector<uint32_t> o(1, 0);
+  for (size_t r = 0; r < dead.size(); ++r)
+    if (!dead[r]) o.push_back(o.back() + (off[r + 1] - off[r]));
+  return o;
+}
+
+template <class T>
+std::vector<T> live_only(const std::vector<T>& v, const std::vector<uint8_t>& dead) {
+  std::vector<T> o;
+  for (size_t r = 0; r < dead.size(); ++r)
+    if (!dead[r]) o.push_back(v[r]);
+  return o;
+}
+
+// The compacted pending table and gate: the host state of the live rows of the handle's,
+// no tombstones, the other device buffers allocated for pending_copy
+int pending_fresh(crane_sched* h, PendingTable& pd, GateRows& g) {
+  const PendingTable& o = h->pd;
+  pd.have_qos_cols = o.have_qos_cols;
+  pd.have_mandated = o.have_mandated;
+  pd.have_pd_resv = o.have_pd_resv;
+  pd.have_lists_incl = o.have_lists_incl;
+  pd.have_lists_excl = o.have_lists_excl;
+  pd.h_alloc_off = live_offsets(o.h_alloc_off, o.h_dead);
+  if (o.have_lists_incl) pd.h_incl_off = live_offsets(o.h_incl_off, o.h_dead);
+  if (o.have_lists_excl) pd.h_excl_off = live_offsets(o.h_excl_off, o.h_dead);
+  pd.h_pd_account = live_only(o.h_pd_account, o.h_dead);
+  pd.total_alloc = pd.h_alloc_off.back();
+  const uint32_t n = o.n - o.n_dead, n1 = std::max<uint32_t>(n, 1);
+  CU(pd.alloc_live(n, h->stream));
+  CU(ensure_cols(pd, n));
+  CU(pd.d_alloc_off.ensure(n1 + 1));
+  if (pd.have_lists_incl) {
+    CU(pd.d_incl_off.ensure(n1 + 1));
+    CU(pd.d_incl_nodes.ensure(std::max<uint32_t>(pd.h_incl_off.back(), 1)));
+  }
+  if (pd.have_lists_excl) {
+    CU(pd.d_excl_off.ensure(n1 + 1));
+    CU(pd.d_excl_nodes.ensure(std::max<uint32_t>(pd.h_excl_off.back(), 1)));
+  }
+  // the gate state of the live rows below the gate's end
+  g.on = h->gate.on;
+  g.h_has_deps = live_only(h->gate.h_has_deps, std::vector<uint8_t>(o.h_dead.begin(), o.h_dead.begin() + h->gate.n));
+  g.n = (uint32_t)g.h_has_deps.size();
+  if (h->gate.n) CU(ensure_cols(g, g.n));
+  return CRANE_OK;
+}
+
+// The live rows of the handle's pending table and gate into the fresh ones (one gather)
+int pending_copy(crane_sched* h, PendingTable& pd, GateRows& g, const uint32_t* live) {
+  PendingTable& o = h->pd;
+  ColSet cs{};
+  o.each(pd, gather_to(cs, pd.n));
+  h->gate.each(g, gather_to(cs, g.n));
+  TRY(gather(h, cs, live, pd.n));
+  TRY(csr_offsets(h, o.d_alloc_off.p, live, pd.n, pd.d_alloc_off.p));
+  if (pd.have_lists_incl) {
+    TRY(csr_offsets(h, o.d_incl_off.p, live, pd.n, pd.d_incl_off.p));
+    TRY(csr_copy(h, o.d_incl_off.p, o.d_incl_nodes.p, live, pd.n, pd.d_incl_off.p, pd.d_incl_nodes.p));
+  }
+  if (pd.have_lists_excl) {
+    TRY(csr_offsets(h, o.d_excl_off.p, live, pd.n, pd.d_excl_off.p));
+    TRY(csr_copy(h, o.d_excl_off.p, o.d_excl_nodes.p, live, pd.n, pd.d_excl_off.p, pd.d_excl_nodes.p));
+  }
+  return CRANE_OK;
+}
+
+// The compacted running table: the host state of the live rows of the handle's, no
+// tombstones, the other device buffers allocated for running_copy
+int running_fresh(crane_sched* h, RunningTable& rr) {
+  const RunningTable& o = h->rr;
+  rr.node_bound = o.node_bound;
+  rr.dirty = o.dirty;  // (the run's view of the running table is the live rows in row order)
+  rr.h_rr_alloc_off = live_offsets(o.h_rr_alloc_off, o.h_dead);
+  rr.h_rr_account = live_only(o.h_rr_account, o.h_dead);
+  const uint32_t n = o.n - o.n_dead, e1 = std::max<uint32_t>(rr.h_rr_alloc_off.back(), 1);
+  CU(rr.alloc_live(n, h->stream));
+  CU(ensure_cols(rr, n));
+  CU(rr.d_rr_alloc_off.ensure((size_t)std::max<uint32_t>(n, 1) + 1));
+  CU(rr.d_rr_alloc_node.ensure(e1));
+  CU(rr.d_rr_alloc_res.ensure(e1));
+  return CRANE_OK;
+}
+
+// The live rows of the handle's running table into the fresh one
+int running_copy(crane_sched* h, RunningTable& rr, const uint32_t* live) {
+  RunningTable& o = h->rr;
+  ColSet cs{};
+  o.each(rr, gather_to(cs, rr.n));
+  TRY(gather(h, cs, live, rr.n));
+  TRY(csr_offsets(h, o.d_rr_alloc_off.p, live, rr.n, rr.d_rr_alloc_off.p));
+  TRY(csr_copy(h, o.d_rr_alloc_off.p, o.d_rr_alloc_node.p, live, rr.n, rr.d_rr_alloc_off.p, rr.d_rr_alloc_node.p));
+  TRY(csr_copy(h, o.d_rr_alloc_off.p, o.d_rr_alloc_res.p, live, rr.n, rr.d_rr_alloc_off.p, rr.d_rr_alloc_res.p));
+  return CRANE_OK;
+}
+
+// ---- the step state of running jobs, resident on the device -------------------------
+
+enum : uint8_t { kSpPending = 0, kSpScheduled = 1, kSpErased = 2 };
+
+void sj_dirty(crane_sched* h, uint32_t j) {
+  if (!h->h_sj_dirty[j]) {
+    h->h_sj_dirty[j] = 1;
+    h->h_sj_dirty_rows.push_back(j);
+  }
+}
+
+// New step-job rows whose nodes and avail are in the pools up to off.back()
+void sj_commit(crane_sched* h, const std::vector<uint32_t>& off) {
+  for (size_t k = 0; k + 1 < off.size(); ++k) {
+    h->h_sj_node_off.push_back(off[k + 1]);
+    h->h_sj_dead.push_back(0);
+    h->h_sj_dirty.push_back(0);
+    h->h_sj_queue.emplace_back();
+    sj_dirty(h, h->n_sj++);
+  }
+}
+
+StepPoolDev step_pool(crane_sched* h) {
+  StepPoolDev p{};
+  p.sj_node_off = h->d_sj_node_off.p;
+  p.sj_node = h->d_sj_node.p;
+  p.sj_avail = h->d_sj_avail.p;
+  p.job = h->d_sp_job.p;
+  p.node_num = h->d_sp_nn.p;
+  p.ntasks = h->d_sp_nt.p;
+  p.ntpn_min = h->d_sp_t0.p;
+  p.ntpn_max = h->d_sp_t1.p;
+  p.req_node = h->d_sp_req_node.p;
+  p.req_task = h->d_sp_req_task.p;
+  p.incl_off = h->d_sp_incl_off.p;
+  p.incl_nodes = h->d_sp_incl.p;
+  p.excl_off = h->d_sp_excl_off.p;
+  p.excl_nodes = h->d_sp_excl.p;
+  p.alloc_at = h->d_sp_alloc_at.p;
+  p.sa_node = h->d_sa_node.p;
+  p.sa_res = h->d_sa_res.p;
+  return p;
+}
+
+// grid of a kernel with one warp per item, 256 threads per block
+uint32_t warp_grid(const crane_sched* h, uint64_t items) {
+  return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((items + 7) / 8, 8ull * h->n_sm));
+}
+
+}  // namespace
+
+extern "C" {
+
+const char* crane_sched_last_error(const crane_sched_t* h) { return h ? h->err.c_str() : "null handle"; }
+
+int crane_sched_create(const crane_sched_config_t* cfg, int device, crane_sched_t** out) {
+  if (!cfg || !out) return CRANE_EINVAL;
+  *out = nullptr;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return CRANE_ENODEV;
+  if (cfg->max_jobs_per_node < 2 || cfg->max_jobs_per_node > 65000) return CRANE_EINVAL;
+  if (cfg->cost_policy > 1) return CRANE_ENOSYS;  // 0 MinCpuTimeRatioFirst (JobScheduler.h:40), 1 BestFit (ours, config 4)
+  if (device >= 64) return CRANE_EINVAL;
+  int slot = -1;
+  {
+    std::lock_guard<std::mutex> lk(g_slot_mu);
+    for (int k = 0; k < kDictSlots; ++k)
+      if (!(g_slots_used[device] >> k & 1u)) { slot = k; g_slots_used[device] |= 1u << k; break; }
+  }
+  if (slot < 0) return CRANE_ENOSYS;  // more than kDictSlots live handles on one device
+  crane_sched* h = new crane_sched();
+  h->cfg = *cfg;
+  h->device = device;
+  h->dict_slot = slot;
+  if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
+    delete h;
+    return CRANE_ENODEV;
+  }
+  for (auto& e : h->ev) cudaEventCreate(&e);
+  int n_sm = 0, smem_optin = 0;
+  if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device) != cudaSuccess ||
+      cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess || n_sm <= 0) {
+    delete h;
+    return CRANE_ENODEV;
+  }
+  h->n_sm = (uint32_t)n_sm;
+  {
+    // k_commit2: everything a block may opt in to (227 KB on H100) beyond the kernel's static tables
+    size_t stat = 20 * 1024;
+#ifndef CRANE_EMU
+    cudaFuncAttributes fa;
+    if (cudaFuncGetAttributes(&fa, k_commit2) == cudaSuccess) stat = fa.sharedSizeBytes;
+#endif
+    const size_t sm_total = (size_t)smem_optin;
+    h->v2_budget = sm_total > stat + 1024 ? sm_total - stat - 1024 : 0;
+    cudaFuncSetAttribute(k_commit2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->v2_budget);
+  }
+  h->tl_cap = cfg->max_jobs_per_node + 1;
+  *out = h;
+  return CRANE_OK;
+}
+
+void crane_sched_destroy(crane_sched_t* h) { delete h; }
 
 int crane_sched_set_cluster(crane_sched_t* h, const crane_cluster_t* c) {
   if (!h || !c) return CRANE_EINVAL;
@@ -736,418 +1493,20 @@ int crane_sched_device_placements(crane_sched_t* h, crane_device_placements_t* o
   out->alloc_node = h->d_out_node.p;
   out->alloc_ntasks = h->d_out_ntasks.p;
   out->alloc_res = h->d_out_res.p;
-  out->n_jobs = h->n_pending;
-  out->n_rows = h->total_alloc;
+  out->n_jobs = h->pd.n;
+  out->n_rows = h->pd.total_alloc;
   return CRANE_OK;
 }
 
-}  // extern "C" (the split upload lives in an unnamed namespace)
-
-namespace {
-
-template <class T>
-int h2d_at(crane_sched* h, DBuf<T>& dst, const T* src, size_t base, size_t n) {
-  CU(dst.grow(std::max<size_t>(base + n, 1), base, h->stream));
-  if (n) CU(cudaMemcpyAsync(dst.p + base, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream));
-  return CRANE_OK;
-}
-#define H2D_AT(buf, src, base, n) TRY(h2d_at(h, buf, src, (size_t)(base), (size_t)(n)))
-
-// Appends the rows of `pd` to the device-resident pending table (rows keep job-id
-// order: the reference's pending map is a btree over job ids, JobScheduler.cpp:1092).
-int pending_append(crane_sched* h, const crane_pending_t* pd) {
-  const uint32_t base = h->n_pending, N = pd->n;
-  if (N && (!pd->partition || !pd->time_limit || !pd->submit_time || !pd->node_num || !pd->ntasks ||
-            !pd->ntasks_per_node_min || !pd->ntasks_per_node_max || !pd->exclusive || !pd->partition_priority ||
-            !pd->qos_priority || !pd->account || !pd->req_node || !pd->req_task || !pd->req_total))
-    return fail(h, CRANE_EINVAL, "pending: null column");
-  if ((uint64_t)base + N > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "pending: too many rows");
-  // optional columns are all-or-nothing over the life of the table
-  if (base) {
-    if ((pd->qos != nullptr && pd->user != nullptr) != h->have_qos_cols || (pd->mandated_priority != nullptr) != h->have_mandated ||
-        (pd->reservation != nullptr) != h->have_pd_resv || (pd->incl_off != nullptr) != h->have_lists_incl ||
-        (pd->excl_off != nullptr) != h->have_lists_excl)
-      return fail(h, CRANE_EINVAL, "pending_append: optional columns (qos/user, mandated_priority, reservation, node lists) must match the table's");
-  } else {
-    h->have_qos_cols = pd->qos != nullptr && pd->user != nullptr;
-    h->have_mandated = pd->mandated_priority != nullptr;
-    h->have_pd_resv = pd->reservation != nullptr;
-    h->have_lists_incl = pd->incl_off != nullptr;
-    h->have_lists_excl = pd->excl_off != nullptr;
-    h->h_alloc_off.assign(1, 0);
-    h->h_incl_off.assign(1, 0);
-    h->h_excl_off.assign(1, 0);
-    h->h_pd_account.clear();
-    h->h_dead.clear();
-    h->n_dead = 0;
-  }
-  // ---- validation + alloc_off (prefix sum of node_num over all rows) -----------
-  uint64_t acc = h->h_alloc_off.back();
-  for (uint32_t i = 0; i < N; ++i) {
-    if (pd->node_num[i] == 0) return fail(h, CRANE_EINVAL, "pending[%u]: node_num == 0", i);
-    if (pd->time_limit[i] < 1) return fail(h, CRANE_EINVAL, "pending[%u]: time_limit < 1", i);
-    const uint32_t t = pd->ntasks_per_node_min[i], tmax = pd->ntasks_per_node_max[i];
-    if (t == 0 || tmax < t) return fail(h, CRANE_EINVAL, "pending[%u]: ntasks_per_node_min/max", i);
-    // general task distribution (the top-K heaps of JobScheduler.cpp:5193-5205): heaps of up to 127 nodes
-    if ((tmax != t || (uint64_t)t * pd->node_num[i] != pd->ntasks[i]) && pd->node_num[i] >= (uint32_t)kHeapMax)
-      return fail(h, CRANE_ENOSYS, "pending[%u]: a job with a ntasks_per_node range wider than %d nodes", i, kHeapMax - 1);
-    if ((uint64_t)tmax * pd->node_num[i] < pd->ntasks[i] || (uint64_t)t * pd->node_num[i] > pd->ntasks[i])
-      return fail(h, CRANE_EINVAL, "pending[%u]: ntasks outside [node_num*ntpn_min, node_num*ntpn_max]", i);
-    if (pd->req_node[i].cpu_raw < 0 || pd->req_task[i].cpu_raw < 0)
-      return fail(h, CRANE_EINVAL, "pending[%u]: negative cpu request", i);
-    if (pd->account[i] > (1u << 24)) return fail(h, CRANE_EINVAL, "account ids must be dense (< 2^24)");
-    acc += pd->node_num[i];
-    if (acc > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "pending: sum(node_num) overflows");
-  }
-  if (pd->incl_off) TRY(check_node_list(h, "pending: include list", pd->incl_off, pd->incl_nodes, N));
-  if (pd->excl_off) TRY(check_node_list(h, "pending: exclude list", pd->excl_off, pd->excl_nodes, N));
-  // ---- columns ----------------------------------------------------------------
-  H2D_AT(h->d_partition, pd->partition, base, N);
-  H2D_AT(h->d_time_limit, pd->time_limit, base, N);
-  H2D_AT(h->d_submit, pd->submit_time, base, N);
-  H2D_AT(h->d_node_num, pd->node_num, base, N);
-  H2D_AT(h->d_ntpn, pd->ntasks_per_node_min, base, N);
-  H2D_AT(h->d_ntpn_max, pd->ntasks_per_node_max, base, N);
-  H2D_AT(h->d_ntasks, pd->ntasks, base, N);
-  H2D_AT(h->d_exclusive, pd->exclusive, base, N);
-  H2D_AT(h->d_part_prio, pd->partition_priority, base, N);
-  H2D_AT(h->d_qos_prio, pd->qos_priority, base, N);
-  H2D_AT(h->d_account, pd->account, base, N);
-  if (h->have_qos_cols) {
-    H2D_AT(h->d_qos, pd->qos, base, N);
-    H2D_AT(h->d_user, pd->user, base, N);
-  }
-  if (h->have_mandated) H2D_AT(h->d_mandated, pd->mandated_priority, base, N);
-  H2D_AT(h->d_req_node, reinterpret_cast<const View*>(pd->req_node), base, N);
-  H2D_AT(h->d_req_task, reinterpret_cast<const View*>(pd->req_task), base, N);
-  H2D_AT(h->d_req_total, reinterpret_cast<const View*>(pd->req_total), base, N);
-  if (h->have_pd_resv) H2D_AT(h->d_pd_resv, pd->reservation, base, N);
-  {
-    std::vector<uint8_t> zeros(N, 0);
-    H2D_AT(h->d_dead, zeros.data(), base, N);
-    CU(cudaStreamSynchronize(h->stream));
-  }
-  // host mirrors
-  for (uint32_t i = 0; i < N; ++i) {
-    h->h_alloc_off.push_back(h->h_alloc_off.back() + pd->node_num[i]);
-    h->h_pd_account.push_back(pd->account[i]);
-    h->h_dead.push_back(0);
-  }
-  H2D_AT(h->d_alloc_off, h->h_alloc_off.data() + base, base, (size_t)N + 1);
-  if (h->have_lists_incl) {
-    const uint32_t nb = h->h_incl_off.back();
-    for (uint32_t i = 0; i < N; ++i) h->h_incl_off.push_back(nb + pd->incl_off[i + 1]);
-    H2D_AT(h->d_incl_off, h->h_incl_off.data() + base, base, (size_t)N + 1);
-    H2D_AT(h->d_incl_nodes, pd->incl_nodes, nb, pd->incl_off[N]);
-  }
-  if (h->have_lists_excl) {
-    const uint32_t nb = h->h_excl_off.back();
-    for (uint32_t i = 0; i < N; ++i) h->h_excl_off.push_back(nb + pd->excl_off[i + 1]);
-    H2D_AT(h->d_excl_off, h->h_excl_off.data() + base, base, (size_t)N + 1);
-    H2D_AT(h->d_excl_nodes, pd->excl_nodes, nb, pd->excl_off[N]);
-  }
-  CU(cudaStreamSynchronize(h->stream));
-  h->n_pending = base + N;
-  h->total_alloc = h->h_alloc_off.back();
-  return CRANE_OK;
-}
-
-// The rows of a host running table: the checks of crane_sched_running_append (`replace`:
-// the rows will replace the table rather than extend it)
-int running_check(crane_sched* h, const crane_running_t* rn, bool replace) {
-  const uint32_t R = rn ? rn->n : 0;
-  if (!R) return CRANE_OK;
-  if (!rn->start_time || !rn->end_time || !rn->node_num || !rn->partition_priority || !rn->qos_priority ||
-      !rn->account || !rn->view_cpu_raw || !rn->view_mem)
-    return fail(h, CRANE_EINVAL, "running: null column");
-  TRY(check_offsets(h, "running: alloc_off", rn->alloc_off, R));
-  const uint32_t E = rn->alloc_off[R];
-  if (E && (!rn->alloc_node || !rn->alloc_res)) return fail(h, CRANE_EINVAL, "running: null allocation table");
-  const uint64_t rows = replace ? 0 : h->n_rr, entries = replace ? 0 : h->h_rr_alloc_off.back();
-  if (rows + R > 0xfffffff0ull || entries + E > 0xfffffff0ull)
-    return fail(h, CRANE_EINVAL, "running: too many rows");
-  for (uint32_t j = 0; j < R; ++j) {
-    if (rn->account[j] > (1u << 24)) return fail(h, CRANE_EINVAL, "account ids must be dense (< 2^24)");
-    for (uint32_t k = rn->alloc_off[j]; k < rn->alloc_off[j + 1]; ++k)
-      if (rn->alloc_node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "running[%u]: node out of range", j);
-  }
-  return CRANE_OK;
-}
-
-void running_reset(crane_sched* h) {
-  h->n_rr = 0;
-  h->n_rr_dead = 0;
-  h->h_rr_alloc_off.assign(1, 0);
-  h->h_rr_account.clear();
-  h->h_rr_dead.clear();
-  h->rr_node_bound = 0;
-  h->rr_dirty = true;
-}
-
-// Appends the rows of a checked host running table to the resident table
-int running_append(crane_sched* h, const crane_running_t* rn) {
-  const uint32_t base = h->n_rr, R = rn ? rn->n : 0;
-  if (!R) return CRANE_OK;
-  const uint32_t eb = h->h_rr_alloc_off.back(), E = rn->alloc_off[R];
-  H2D_AT(h->d_rr_start, rn->start_time, base, R);
-  H2D_AT(h->d_rr_end, rn->end_time, base, R);
-  H2D_AT(h->d_rr_node_num, rn->node_num, base, R);
-  H2D_AT(h->d_rr_part_prio, rn->partition_priority, base, R);
-  H2D_AT(h->d_rr_qos_prio, rn->qos_priority, base, R);
-  H2D_AT(h->d_rr_account, rn->account, base, R);
-  H2D_AT(h->d_rr_cpu, rn->view_cpu_raw, base, R);
-  H2D_AT(h->d_rr_mem, rn->view_mem, base, R);
-  std::vector<uint32_t> no_resv(rn->reservation ? 0 : R, 0xffffffffu);
-  H2D_AT(h->d_rr_resv, rn->reservation ? rn->reservation : no_resv.data(), base, R);
-  std::vector<uint8_t> zeros(R, 0);
-  H2D_AT(h->d_rr_dead, zeros.data(), base, R);
-  for (uint32_t j = 0; j < R; ++j) {
-    h->h_rr_alloc_off.push_back(eb + rn->alloc_off[j + 1]);
-    h->h_rr_account.push_back(rn->account[j]);
-    h->h_rr_dead.push_back(0);
-  }
-  H2D_AT(h->d_rr_alloc_off, h->h_rr_alloc_off.data() + base, base, (size_t)R + 1);
-  H2D_AT(h->d_rr_alloc_node, rn->alloc_node, eb, E);
-  H2D_AT(h->d_rr_alloc_res, reinterpret_cast<const Row*>(rn->alloc_res), eb, E);
-  for (uint32_t k = 0; k < E; ++k) h->rr_node_bound = std::max(h->rr_node_bound, rn->alloc_node[k] + 1);
-  CU(cudaStreamSynchronize(h->stream));  // (the staging vectors are pageable)
-  h->n_rr = base + R;
-  h->rr_dirty = true;
-  return CRANE_OK;
-}
-
-RunTableDev run_table(crane_sched* h) {
-  RunTableDev rt{};
-  rt.n = h->n_rr;
-  rt.start_time = h->d_rr_start.p;
-  rt.end_time = h->d_rr_end.p;
-  rt.node_num = h->d_rr_node_num.p;
-  rt.partition_priority = h->d_rr_part_prio.p;
-  rt.qos_priority = h->d_rr_qos_prio.p;
-  rt.account = h->d_rr_account.p;
-  rt.reservation = h->d_rr_resv.p;
-  rt.view_cpu_raw = h->d_rr_cpu.p;
-  rt.view_mem = h->d_rr_mem.p;
-  rt.alloc_off = h->d_rr_alloc_off.p;
-  rt.alloc_node = h->d_rr_alloc_node.p;
-  rt.alloc_res = h->d_rr_alloc_res.p;
-  rt.dead = h->d_rr_dead.p;
-  return rt;
-}
-
-// The tick's RunningDev view of the live rows, on the device: the dense per-job columns
-// (live rows in row order), the allocations grouped by node state and the jobs grouped by
-// account, both stable (order inside a node state / account is row order, deviation D6).
-int regroup(crane_sched* h, uint32_t R, uint32_t max_rn_account) {
-  cudaStream_t st = h->stream;
-  const uint32_t Rt = h->n_rr, E = h->h_rr_alloc_off.back();
-  const RunTableDev rt = run_table(h);
-  CU(h->d_rn_start.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_end.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_node_num.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_part_prio.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_qos_prio.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_account.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_cpu.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_mem.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_acc_key.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_acc_job.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_slot_off.ensure((size_t)h->n_slots + 1));
-  CU(h->d_rn_slot_end.ensure(std::max<uint32_t>(E, 1)));
-  CU(h->d_rn_slot_res.ensure(std::max<uint32_t>(E, 1)));
-  CU(h->d_flag.ensure(1));
-  CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
-  uint64_t* keys;
-  uint32_t* vals;
-  // live rows in row order -> the dense columns (without tombstones: every row, in order)
-  if (R) {
-    vals = nullptr;
-    if (h->n_rr_dead) {
-      CRANE_LAUNCH(k_rt_live_keys, (Rt + 255) / 256, 256, 0, st, rt.dead, Rt, h->d_keys_a.p, h->d_vals_a.p);
-      TRY(radix_sort(h, Rt, 8, &keys, &vals));
-    }
-    const RunningCols o{h->d_rn_start.p, h->d_rn_end.p, h->d_rn_node_num.p, h->d_rn_part_prio.p,
-                        h->d_rn_qos_prio.p, h->d_rn_account.p, h->d_rn_cpu.p, h->d_rn_mem.p};
-    CRANE_LAUNCH(k_rt_gather, (R + 255) / 256, 256, 0, st, rt, vals, R, o);
-  }
-  // allocations by node state: stable sort of the entries (row order) by slot
-  if (E) {
-    NodeStateMap m{h->n_nodes, h->n_slots, h->n_comp, h->n_resv, h->d_node_slot.p, h->d_part_base.p, h->d_r_node_off.p, h->d_r_node.p};
-    const uint32_t nb = std::min<uint32_t>((Rt + 7) / 8, 8 * h->n_sm);
-    CRANE_LAUNCH(k_rt_entry_keys, nb, 256, 0, st, rt, m, h->d_keys_a.p, h->d_vals_a.p, h->d_flag.p);
-    int bits = 8;
-    while ((1ull << bits) <= (uint64_t)h->n_slots) bits += 8;
-    TRY(radix_sort(h, E, bits, &keys, &vals));
-    CRANE_LAUNCH(k_rt_offsets, (h->n_slots + 1 + 255) / 256, 256, 0, st, keys, E, h->n_slots, h->d_rn_slot_off.p);
-    CRANE_LAUNCH(k_rt_slot_gather, (E + 255) / 256, 256, 0, st, rt, keys, vals, E, h->d_rn_slot_off.p + h->n_slots,
-                 h->d_rn_slot_end.p, h->d_rn_slot_res.p);
-  } else {
-    CU(cudaMemsetAsync(h->d_rn_slot_off.p, 0, sizeof(uint32_t) * ((size_t)h->n_slots + 1), st));
-  }
-  // jobs by account: stable sort of the view's jobs by account
-  if (R) {
-    CRANE_LAUNCH(k_rt_acc_keys, (R + 255) / 256, 256, 0, st, h->d_rn_account.p, R, h->d_keys_a.p, h->d_vals_a.p);
-    int bits = 8;
-    while ((1ull << bits) <= (uint64_t)max_rn_account) bits += 8;
-    TRY(radix_sort(h, R, bits, &keys, &vals));
-    CU(cudaMemcpyAsync(h->d_rn_acc_key.p, keys, sizeof(uint64_t) * R, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(h->d_rn_acc_job.p, vals, sizeof(uint32_t) * R, cudaMemcpyDeviceToDevice, st));
-  }
-  CU(cudaGetLastError());
-  // a cluster with fewer nodes than the rows name: one flag read back
-  if (E && h->rr_node_bound > h->n_nodes) {
-    uint32_t bad = 0;
-    CU(cudaMemcpyAsync(&bad, h->d_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    if (bad) return fail(h, CRANE_EINVAL, "running: node out of range");
-  }
-  h->rr_dirty = false;
-  return CRANE_OK;
-}
-
-// "The next run uses the running table as it stands on the device": the view of the
-// live rows (regrouped when the rows or the node-state layout changed) and the work and
-// output buffers for the resident pending table.
-int keep_running(crane_sched* h) {
-  cudaStream_t st = h->stream;
-  const uint32_t N = h->n_pending, Rt = h->n_rr, R = Rt - h->n_rr_dead;
-  const uint32_t E = h->h_rr_alloc_off.back();
-  uint32_t max_rn_account = 0, max_account = 0;
-  for (uint32_t r = 0; r < Rt; ++r)
-    if (!h->h_rr_dead[r]) max_rn_account = std::max(max_rn_account, h->h_rr_account[r]);
-  for (uint32_t i = 0; i < N; ++i) max_account = std::max(max_account, h->h_pd_account[i]);
-  max_account = std::max(max_account, max_rn_account);
-  const uint32_t A = (N + R) ? max_account + 1 : 0;
-
-  // ---- work + output buffers (the sorts of the regroup use the priority sort's) ----
-  size_t n1 = std::max<uint32_t>(N, 1);
-  const size_t ns = std::max<size_t>({n1, (size_t)Rt, (size_t)E});
-  CU(h->d_bounds.ensure(1));
-  CU(h->d_acc_service.ensure(std::max<uint32_t>(A, 1)));
-  CU(h->d_prio.ensure(n1));
-  CU(h->d_keys_a.ensure(ns));
-  CU(h->d_keys_b.ensure(ns));
-  CU(h->d_vals_a.ensure(ns));
-  CU(h->d_vals_b.ensure(ns));
-  uint32_t nq = std::min<uint32_t>(N, h->cfg.scheduled_batch_size);
-  CU(h->d_jobq.ensure(std::max<uint32_t>(nq, 1)));
-  CU(h->d_bitmap.ensure((size_t)std::max<uint32_t>(nq, 1) * h->words_per_row));
-  CU(h->d_reason.ensure(n1));
-  CU(h->d_out_prio.ensure(n1));
-  CU(h->d_out_start.ensure(n1));
-  CU(h->d_out_end.ensure(n1));
-  CU(h->d_out_nalloc.ensure(n1));
-  size_t ta = std::max<uint64_t>(h->total_alloc, 1);
-  CU(h->d_out_node.ensure(ta));
-  CU(h->d_out_ntasks.ensure(ta));
-  CU(h->d_out_res.ensure(ta));
-
-  CU(cudaEventRecord(h->ev[kEvKeepBegin], st));
-  if (h->rr_dirty) TRY(regroup(h, R, max_rn_account));
-  // ---- accounts: offsets of the account groups, accounts present (pending included) ----
-  CU(h->d_rn_acc_off.ensure((size_t)A + 1));
-  CU(h->d_acc_present.ensure(std::max<uint32_t>(A, 1)));
-  CRANE_LAUNCH(k_rt_offsets, (A + 1 + 255) / 256, 256, 0, st, h->d_rn_acc_key.p, R, A, h->d_rn_acc_off.p);
-  CU(cudaMemsetAsync(h->d_acc_present.p, 0, std::max<uint32_t>(A, 1), st));
-  if (N + R)
-    CRANE_LAUNCH(k_acc_present, (N + R + 255) / 256, 256, 0, st, h->d_account.p, h->n_dead ? h->d_dead.p : nullptr, N,
-                 h->d_rn_account.p, R, h->d_acc_present.p);
-  CU(cudaEventRecord(h->ev[kEvKeepEnd], st));
-  CU(cudaGetLastError());
-  h->n_running = R;
-  h->n_accounts = A;
-  return CRANE_OK;
-}
-
-// The running table of this tick from a host table: reset + append + keep_running
-int set_running(crane_sched* h, const crane_running_t* rn) {
-  TRY(running_check(h, rn, true));
-  running_reset(h);
-  TRY(running_append(h, rn));
-  return keep_running(h);
-}
-
-GateDev gate_dev(crane_sched* h) {
-  GateDev g{};
-  g.n = h->gate_n;
-  g.dead = h->n_dead ? h->d_dead.p : nullptr;
-  g.held = h->d_g_held.p;
-  g.begin = h->d_g_begin.p;
-  g.is_or = h->d_g_is_or.p;
-  g.open = h->d_g_open.p;
-  g.ready = h->d_g_ready.p;
-  g.n_ent = h->n_ent;
-  g.dependent = h->d_e_dependent.p;
-  g.dependee = h->d_e_dependee.p;
-  g.kind = h->d_e_kind.p;
-  g.type = h->d_e_type.p;
-  g.live = h->d_e_live.p;
-  g.delay = h->d_e_delay.p;
-  return g;
-}
-
-// Turns the gate on and gives the rows appended since the last gate call their state:
-// not held, beginning at InfinitePast, no dependencies
-int gate_fit(crane_sched* h) {
-  h->gate_on = true;
-  const uint32_t from = h->gate_n, to = h->n_pending;
-  if (to <= from) return CRANE_OK;
-  cudaStream_t st = h->stream;
-  CU(h->d_g_held.grow(to, from, st));
-  CU(h->d_g_begin.grow(to, from, st));
-  CU(h->d_g_is_or.grow(to, from, st));
-  CU(h->d_g_open.grow(to, from, st));
-  CU(h->d_g_ready.grow(to, from, st));
-  h->gate_n = to;
-  h->h_has_deps.resize(to, 0);
-  CRANE_LAUNCH(k_gate_init, (to - from + 255) / 256, 256, 0, st, gate_dev(h), from, to);
-  CU(cudaGetLastError());
-  return CRANE_OK;
-}
-
-// The rows of a call on the device, sorted, followed by their places in the call's list
-int upload_call_rows(crane_sched* h, const uint32_t* rows, uint32_t n) {
-  std::vector<uint32_t> idx(n), buf(2 * (size_t)n);
-  for (uint32_t k = 0; k < n; ++k) idx[k] = k;
-  std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return rows[a] < rows[b]; });
-  for (uint32_t k = 0; k < n; ++k) {
-    buf[k] = rows[idx[k]];
-    buf[n + k] = idx[k];
-  }
-  H2D(h->d_ev_rows, buf.data(), buf.size());
-  CU(cudaStreamSynchronize(h->stream));  // (buf is pageable)
-  return CRANE_OK;
-}
-
-// k_dep_fire over `threads` entries for the events of the call whose rows upload_call_rows placed
-int dep_fire(crane_sched* h, DepEvents ev, uint32_t n_rows, uint32_t threads) {
-  if (!threads) return CRANE_OK;
-  ev.n = n_rows;
-  ev.rows = h->d_ev_rows.p;
-  ev.pos = h->d_ev_rows.p + n_rows;
-  CRANE_LAUNCH(k_dep_fire, (threads + 255) / 256, 256, 0, h->stream, gate_dev(h), ev);
-  CU(cudaGetLastError());
-  return CRANE_OK;
-}
-
-}  // namespace
-
-extern "C" {
-
-uint32_t crane_sched_pending_rows(const crane_sched_t* h) { return h ? h->n_pending : 0; }
+uint32_t crane_sched_pending_rows(const crane_sched_t* h) { return h ? h->pd.n : 0; }
 
 int crane_sched_pending_reset(crane_sched_t* h) {
   if (!h) return CRANE_EINVAL;
-  h->n_pending = 0;
-  h->total_alloc = 0;
-  h->n_dead = 0;
-  h->h_alloc_off.assign(1, 0);
-  h->h_pd_account.clear();
-  h->h_dead.clear();
-  h->gate_on = false;
-  h->gate_n = 0;
-  h->h_has_deps.clear();
-  h->n_ent = 0;
+  h->pd.reset();
+  h->gate.on = false;
+  h->gate.n = 0;
+  h->gate.h_has_deps.clear();
+  h->ent.n = 0;
   lower_stage(h, kCluster);
   return CRANE_OK;
 }
@@ -1157,29 +1516,18 @@ int crane_sched_pending_append(crane_sched_t* h, const crane_pending_t* rows, ui
   TRY(require(h, kCluster, "pending_append"));
   CU(cudaSetDevice(h->device));
   lower_stage(h, kCluster);  // the running table and the work buffers follow with crane_sched_set_running
-  const uint32_t base = h->n_pending;
+  const uint32_t base = h->pd.n;
   TRY(pending_append(h, rows));
   if (first_row) *first_row = base;
   return CRANE_OK;
 }
 
 int crane_sched_pending_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n) {
-  if (!h || (n && !rows)) return CRANE_EINVAL;
-  CU(cudaSetDevice(h->device));
-  for (uint32_t k = 0; k < n; ++k)
-    if (rows[k] >= h->n_pending) return fail(h, CRANE_EINVAL, "pending_erase: row %u out of range", rows[k]);
-  lower_stage(h, kCluster);
-  if (!n) return CRANE_OK;
-  for (uint32_t k = 0; k < n; ++k)
-    if (!h->h_dead[rows[k]]) { h->h_dead[rows[k]] = 1; h->n_dead++; }
-  H2D(h->d_erase_rows, rows, n);
-  CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, h->stream, h->d_erase_rows.p, n, h->d_dead.p);
-  CU(cudaGetLastError());
-  CU(cudaStreamSynchronize(h->stream));
-  return CRANE_OK;
+  if (!h) return CRANE_EINVAL;
+  return erase_rows(h, "pending_erase", h->pd, rows, n);
 }
 
-uint32_t crane_sched_running_rows(const crane_sched_t* h) { return h ? h->n_rr : 0; }
+uint32_t crane_sched_running_rows(const crane_sched_t* h) { return h ? h->rr.n : 0; }
 
 int crane_sched_running_append(crane_sched_t* h, const crane_running_t* rows, uint32_t* first_row) {
   if (!h || !rows) return CRANE_EINVAL;
@@ -1187,26 +1535,16 @@ int crane_sched_running_append(crane_sched_t* h, const crane_running_t* rows, ui
   CU(cudaSetDevice(h->device));
   TRY(running_check(h, rows, false));
   lower_stage(h, kCluster);  // the next run needs crane_sched_keep_running
-  const uint32_t base = h->n_rr;
+  const uint32_t base = h->rr.n;
   TRY(running_append(h, rows));
   if (first_row) *first_row = base;
   return CRANE_OK;
 }
 
 int crane_sched_running_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n) {
-  if (!h || (n && !rows)) return CRANE_EINVAL;
-  CU(cudaSetDevice(h->device));
-  for (uint32_t k = 0; k < n; ++k)
-    if (rows[k] >= h->n_rr) return fail(h, CRANE_EINVAL, "running_erase: row %u out of range", rows[k]);
-  lower_stage(h, kCluster);
-  if (!n) return CRANE_OK;
-  for (uint32_t k = 0; k < n; ++k)
-    if (!h->h_rr_dead[rows[k]]) { h->h_rr_dead[rows[k]] = 1; h->n_rr_dead++; }
-  H2D(h->d_erase_rows, rows, n);
-  CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, h->stream, h->d_erase_rows.p, n, h->d_rr_dead.p);
-  CU(cudaGetLastError());
-  CU(cudaStreamSynchronize(h->stream));
-  h->rr_dirty = true;
+  if (!h) return CRANE_EINVAL;
+  TRY(erase_rows(h, "running_erase", h->rr, rows, n));
+  if (n) h->rr.dirty = true;
   return CRANE_OK;
 }
 
@@ -1217,20 +1555,12 @@ int crane_sched_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32
   TRY(require(h, kRan, "start"));
   CU(cudaSetDevice(h->device));
   cudaStream_t st = h->stream;
-  const uint32_t base = h->n_rr, eb = h->h_rr_alloc_off.back();
-  {
-    std::vector<uint32_t> sorted(rows, rows + n);
-    std::sort(sorted.begin(), sorted.end());
-    for (uint32_t k = 0; k < n; ++k) {
-      if (sorted[k] >= h->n_pending) return fail(h, CRANE_EINVAL, "start: row %u out of range", sorted[k]);
-      if (h->h_dead[sorted[k]]) return fail(h, CRANE_EINVAL, "start: row %u was erased", sorted[k]);
-      if (k && sorted[k] == sorted[k - 1]) return fail(h, CRANE_EINVAL, "start: row %u listed twice", sorted[k]);
-    }
-  }
+  const uint32_t base = h->rr.n, eb = h->rr.h_rr_alloc_off.back();
+  TRY(check_rows(h, "start", rows, n, h->pd.n, [&](uint32_t r) { return h->pd.h_dead[r] != 0; }));
   // the new rows' allocation offsets: node_num of the started rows (host mirror of alloc_off)
   std::vector<uint32_t> off(n + 1, eb);
   for (uint32_t k = 0; k < n; ++k) {
-    const uint64_t e = (uint64_t)off[k] + (h->h_alloc_off[rows[k] + 1] - h->h_alloc_off[rows[k]]);
+    const uint64_t e = (uint64_t)off[k] + (h->pd.h_alloc_off[rows[k] + 1] - h->pd.h_alloc_off[rows[k]]);
     if (e > 0xfffffff0ull || (uint64_t)base + n > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "start: too many running rows");
     off[k + 1] = (uint32_t)e;
   }
@@ -1252,56 +1582,40 @@ int crane_sched_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32
     return CRANE_OK;
   }
   const uint32_t rows_end = base + n, ent_end = off[n];
-  CU(h->d_rr_start.grow(rows_end, base, st));
-  CU(h->d_rr_end.grow(rows_end, base, st));
-  CU(h->d_rr_node_num.grow(rows_end, base, st));
-  CU(h->d_rr_part_prio.grow(rows_end, base, st));
-  CU(h->d_rr_qos_prio.grow(rows_end, base, st));
-  CU(h->d_rr_account.grow(rows_end, base, st));
-  CU(h->d_rr_resv.grow(rows_end, base, st));
-  CU(h->d_rr_cpu.grow(rows_end, base, st));
-  CU(h->d_rr_mem.grow(rows_end, base, st));
-  CU(h->d_rr_alloc_node.grow(ent_end, eb, st));
-  CU(h->d_rr_alloc_res.grow(ent_end, eb, st));
-  H2D_AT(h->d_rr_alloc_off, off.data(), base, (size_t)n + 1);
+  CU(grow_cols(h->rr, rows_end, base, st));
+  CU(h->rr.d_rr_alloc_node.grow(ent_end, eb, st));
+  CU(h->rr.d_rr_alloc_res.grow(ent_end, eb, st));
+  H2D_AT(h->rr.d_rr_alloc_off, off.data(), base, (size_t)n + 1);
   std::vector<uint8_t> zeros(n, 0);
-  H2D_AT(h->d_rr_dead, zeros.data(), base, n);
-  PendingDev pd{};
-  pd.node_num = h->d_node_num.p;
-  pd.alloc_off = h->d_alloc_off.p;
-  pd.partition_priority = h->d_part_prio.p;
-  pd.qos_priority = h->d_qos_prio.p;
-  pd.account = h->d_account.p;
-  pd.reservation = h->have_pd_resv ? h->d_pd_resv.p : nullptr;
+  H2D_AT(h->rr.d_dead, zeros.data(), base, n);
   PlaceDev out{};
   out.start_time = h->d_out_start.p;
   out.end_time = h->d_out_end.p;
   out.alloc_node = h->d_out_node.p;
   out.alloc_res = h->d_out_res.p;
-  RunTableDev rt = run_table(h);
   const uint32_t nb = std::min<uint32_t>((n + 7) / 8, 8 * h->n_sm);
-  CRANE_LAUNCH(k_start, nb, 256, 0, st, pd, out, h->d_start_rows.p, n, base, rt);
+  CRANE_LAUNCH(k_start, nb, 256, 0, st, h->pd.dev(), out, h->d_start_rows.p, n, base, h->rr.dev());
   // the pending rows leave the pending table (m_pending_job_map_.erase, JobScheduler.cpp:1305)
-  CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, st, h->d_start_rows.p, n, h->d_dead.p);
+  CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, st, h->d_start_rows.p, n, h->pd.d_dead.p);
   CU(cudaGetLastError());
-  if (h->n_ent) {  // AFTER fires at the placement's start (JobScheduler.cpp:1549), the rest follow the job
+  if (h->ent.n) {  // AFTER fires at the placement's start (JobScheduler.cpp:1549), the rest follow the job
     TRY(upload_call_rows(h, rows, n));
     DepEvents ev{};
     ev.mode = kFireStart;
     ev.time = h->d_out_start.p;
     ev.base = base;
-    TRY(dep_fire(h, ev, n, h->n_ent));
+    TRY(dep_fire(h, ev, n, h->ent.n));
   }
   for (uint32_t k = 0; k < n; ++k) {
-    h->h_dead[rows[k]] = 1;
-    h->h_rr_account.push_back(h->h_pd_account[rows[k]]);
-    h->h_rr_dead.push_back(0);
-    h->h_rr_alloc_off.push_back(off[k + 1]);
+    h->pd.h_dead[rows[k]] = 1;
+    h->rr.h_rr_account.push_back(h->pd.h_pd_account[rows[k]]);
+    h->rr.h_dead.push_back(0);
+    h->rr.h_rr_alloc_off.push_back(off[k + 1]);
   }
-  h->n_dead += n;
-  h->n_rr = rows_end;
-  h->rr_node_bound = std::max(h->rr_node_bound, h->n_nodes);  // (placements are on this cluster's nodes)
-  h->rr_dirty = true;
+  h->pd.n_dead += n;
+  h->rr.n = rows_end;
+  h->rr.node_bound = std::max(h->rr.node_bound, h->n_nodes);  // (placements are on this cluster's nodes)
+  h->rr.dirty = true;
   CU(cudaStreamSynchronize(st));
   if (first_row) *first_row = base;
   return CRANE_OK;
@@ -1313,7 +1627,7 @@ int crane_sched_pending_set_gate(crane_sched_t* h, const uint32_t* rows, uint32_
   TRY(require(h, kCluster, "pending_set_gate"));
   CU(cudaSetDevice(h->device));
   for (uint32_t k = 0; k < n; ++k)
-    if (rows[k] >= h->n_pending) return fail(h, CRANE_EINVAL, "pending_set_gate: row %u out of range", rows[k]);
+    if (rows[k] >= h->pd.n) return fail(h, CRANE_EINVAL, "pending_set_gate: row %u out of range", rows[k]);
   lower_stage(h, kCluster);
   TRY(gate_fit(h));
   if (n && (held || begin_time)) {
@@ -1337,7 +1651,7 @@ int crane_sched_pending_depend(crane_sched_t* h, const crane_dependencies_t* d) 
   TRY(check_offsets(h, "depend: dep_off", d->dep_off, n));
   const uint32_t m = d->dep_off[n];
   if (m && (!d->kind || !d->dependee || !d->type || !d->delay_s)) return fail(h, CRANE_EINVAL, "depend: null entry column");
-  if ((uint64_t)h->n_ent + m > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "depend: too many entries");
+  if ((uint64_t)h->ent.n + m > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "depend: too many entries");
   {
     std::vector<uint32_t> sorted(d->row, d->row + n);
     std::sort(sorted.begin(), sorted.end());
@@ -1347,9 +1661,9 @@ int crane_sched_pending_depend(crane_sched_t* h, const crane_dependencies_t* d) 
   std::vector<uint32_t> dependent(m), dependee(m);
   for (uint32_t k = 0; k < n; ++k) {
     const uint32_t r = d->row[k];
-    if (r >= h->n_pending) return fail(h, CRANE_EINVAL, "depend: row %u out of range", r);
-    if (h->h_dead[r]) return fail(h, CRANE_EINVAL, "depend: row %u was erased", r);
-    if (r < h->h_has_deps.size() && h->h_has_deps[r]) return fail(h, CRANE_EINVAL, "depend: row %u already has its list", r);
+    if (r >= h->pd.n) return fail(h, CRANE_EINVAL, "depend: row %u out of range", r);
+    if (h->pd.h_dead[r]) return fail(h, CRANE_EINVAL, "depend: row %u was erased", r);
+    if (r < h->gate.h_has_deps.size() && h->gate.h_has_deps[r]) return fail(h, CRANE_EINVAL, "depend: row %u already has its list", r);
     for (uint32_t e = d->dep_off[k]; e < d->dep_off[k + 1]; ++e) {
       const uint8_t kind = d->kind[e];
       const uint32_t q = d->dependee[e];
@@ -1359,9 +1673,9 @@ int crane_sched_pending_depend(crane_sched_t* h, const crane_dependencies_t* d) 
       if (kind == CRANE_DEPENDEE_EVENT) {
         if (!d->event_time) return fail(h, CRANE_EINVAL, "depend: EVENT entries without event_time");
       } else if (kind == CRANE_DEPENDEE_PENDING) {
-        if (q >= h->n_pending || h->h_dead[q]) return fail(h, CRANE_EINVAL, "depend: row %u: pending dependee %u missing", r, q);
+        if (q >= h->pd.n || h->pd.h_dead[q]) return fail(h, CRANE_EINVAL, "depend: row %u: pending dependee %u missing", r, q);
         if (q == r) return fail(h, CRANE_EINVAL, "depend: row %u depends on itself", r);
-      } else if (q >= h->n_rr || h->h_rr_dead[q]) {
+      } else if (q >= h->rr.n || h->rr.h_dead[q]) {
         return fail(h, CRANE_EINVAL, "depend: row %u: running dependee %u missing", r, q);
       }
       for (uint32_t e2 = d->dep_off[k]; e2 < e && kind != CRANE_DEPENDEE_EVENT; ++e2)  // `deps` is a map
@@ -1373,19 +1687,19 @@ int crane_sched_pending_depend(crane_sched_t* h, const crane_dependencies_t* d) 
   lower_stage(h, kCluster);
   TRY(gate_fit(h));
   cudaStream_t st = h->stream;
-  const uint32_t e0 = h->n_ent;
+  const uint32_t e0 = h->ent.n;
   if (m) {
     std::vector<uint8_t> live(m, 1);
-    H2D_AT(h->d_e_dependent, dependent.data(), e0, m);
-    H2D_AT(h->d_e_dependee, dependee.data(), e0, m);
-    H2D_AT(h->d_e_kind, d->kind, e0, m);
-    H2D_AT(h->d_e_type, d->type, e0, m);
-    H2D_AT(h->d_e_delay, d->delay_s, e0, m);
-    H2D_AT(h->d_e_live, live.data(), e0, m);
+    H2D_AT(h->ent.d_e_dependent, dependent.data(), e0, m);
+    H2D_AT(h->ent.d_e_dependee, dependee.data(), e0, m);
+    H2D_AT(h->ent.d_e_kind, d->kind, e0, m);
+    H2D_AT(h->ent.d_e_type, d->type, e0, m);
+    H2D_AT(h->ent.d_e_delay, d->delay_s, e0, m);
+    H2D_AT(h->ent.d_e_live, live.data(), e0, m);
     if (d->event_time) H2D(h->d_ev_i64, d->event_time, m);
     CU(cudaStreamSynchronize(st));  // (the staging vectors are pageable)
   }
-  h->n_ent = e0 + m;
+  h->ent.n = e0 + m;
   if (n) {
     H2D(h->d_ev_rows, d->row, n);
     H2D(h->d_ev_u8, d->is_or, n);
@@ -1396,23 +1710,23 @@ int crane_sched_pending_depend(crane_sched_t* h, const crane_dependencies_t* d) 
   // entries resolved on arrival: EVENT, and AFTER on a running dependee
   DepEvents ev{};
   ev.mode = kFireDepend;
-  ev.run_start = h->d_rr_start.p;
+  ev.run_start = h->rr.d_rr_start.p;
   ev.event_time = d->event_time ? h->d_ev_i64.p : nullptr;
   ev.e0 = e0;
   TRY(dep_fire(h, ev, 0, m));
-  for (uint32_t k = 0; k < n; ++k) h->h_has_deps[d->row[k]] = 1;
+  for (uint32_t k = 0; k < n; ++k) h->gate.h_has_deps[d->row[k]] = 1;
   CU(cudaStreamSynchronize(st));
   return CRANE_OK;
 }
 
 int crane_sched_pending_cancel(crane_sched_t* h, const uint32_t* rows, uint32_t n, int64_t cancel_time) {
   TRY(crane_sched_pending_erase(h, rows, n));
-  if (!n || !h->n_ent) return CRANE_OK;
+  if (!n || !h->ent.n) return CRANE_OK;
   TRY(upload_call_rows(h, rows, n));
   DepEvents ev{};
   ev.mode = kFireCancel;
   ev.t = cancel_time;
-  TRY(dep_fire(h, ev, n, h->n_ent));
+  TRY(dep_fire(h, ev, n, h->ent.n));
   CU(cudaStreamSynchronize(h->stream));
   return CRANE_OK;
 }
@@ -1422,7 +1736,7 @@ int crane_sched_running_end(crane_sched_t* h, const uint32_t* rows, uint32_t n, 
   if (!h) return CRANE_EINVAL;
   if (n && (!end_time || !exit_code)) return fail(h, CRANE_EINVAL, "running_end: null column");
   TRY(crane_sched_running_erase(h, rows, n));
-  if (!n || !h->n_ent) return CRANE_OK;
+  if (!n || !h->ent.n) return CRANE_OK;
   TRY(upload_call_rows(h, rows, n));
   H2D(h->d_ev_i64, end_time, n);
   H2D(h->d_ev_u32, exit_code, n);
@@ -1430,65 +1744,10 @@ int crane_sched_running_end(crane_sched_t* h, const uint32_t* rows, uint32_t n, 
   ev.mode = kFireEnd;
   ev.time = h->d_ev_i64.p;
   ev.code = h->d_ev_u32.p;
-  TRY(dep_fire(h, ev, n, h->n_ent));
+  TRY(dep_fire(h, ev, n, h->ent.n));
   CU(cudaStreamSynchronize(h->stream));
   return CRANE_OK;
 }
-
-}  // extern "C" (the compaction's helpers live in an unnamed namespace)
-
-namespace {
-
-// The live rows of a table of n rows, in row order (the stable sort by tombstone flag),
-// into live[0, n_live), and the old -> new map into map[0, n)
-int live_rows(crane_sched* h, const uint8_t* dead, uint32_t n, uint32_t n_live, uint32_t* live, uint32_t* map) {
-  cudaStream_t st = h->stream;
-  uint64_t* keys;
-  uint32_t* vals;
-  CRANE_LAUNCH(k_rt_live_keys, (n + 255) / 256, 256, 0, st, dead, n, h->d_keys_a.p, h->d_vals_a.p);
-  TRY(radix_sort(h, n, 8, &keys, &vals));
-  if (n_live) CU(cudaMemcpyAsync(live, vals, sizeof(uint32_t) * n_live, cudaMemcpyDeviceToDevice, st));
-  CU(cudaMemsetAsync(map, 0xff, sizeof(uint32_t) * n, st));
-  if (n_live) CRANE_LAUNCH(k_cp_map, (n_live + 255) / 256, 256, 0, st, live, n_live, map);
-  return CRANE_OK;
-}
-
-// new_off[0, n_live] = the offsets of the live rows of a CSR table
-int csr_offsets(crane_sched* h, const uint32_t* off, const uint32_t* live, uint32_t n_live, uint32_t* new_off) {
-  CRANE_LAUNCH(k_cp_lengths, (n_live + 1 + 255) / 256, 256, 0, h->stream, off, live, n_live, new_off);
-  CRANE_LAUNCH(k_sort_scan, 1, 1024, 0, h->stream, new_off, n_live + 1);
-  return CRANE_OK;
-}
-
-// The entries of the live rows of a CSR table at their new offsets
-template <class T>
-int csr_copy(crane_sched* h, const uint32_t* off, const T* src, const uint32_t* live, uint32_t n_live,
-             const uint32_t* new_off, T* dst) {
-  if (!n_live) return CRANE_OK;
-  const uint32_t nb = std::min<uint32_t>((n_live + 7) / 8, 8 * h->n_sm);
-  CRANE_LAUNCH(k_cp_csr<T>, nb, 256, 0, h->stream, off, src, live, n_live, new_off, dst);
-  return CRANE_OK;
-}
-
-// Host mirror of a CSR table's offsets for its live rows
-std::vector<uint32_t> live_offsets(const std::vector<uint32_t>& off, const std::vector<uint8_t>& dead) {
-  std::vector<uint32_t> o(1, 0);
-  for (size_t r = 0; r < dead.size(); ++r)
-    if (!dead[r]) o.push_back(o.back() + (off[r + 1] - off[r]));
-  return o;
-}
-
-template <class T>
-std::vector<T> live_only(const std::vector<T>& v, const std::vector<uint8_t>& dead) {
-  std::vector<T> o;
-  for (size_t r = 0; r < dead.size(); ++r)
-    if (!dead[r]) o.push_back(v[r]);
-  return o;
-}
-
-}  // namespace
-
-extern "C" {
 
 int crane_sched_compact(crane_sched_t* h, uint32_t* pending_map, uint32_t* running_map) {
   if (!h) return CRANE_EINVAL;
@@ -1496,11 +1755,9 @@ int crane_sched_compact(crane_sched_t* h, uint32_t* pending_map, uint32_t* runni
   CU(cudaSetDevice(h->device));
   lower_stage(h, kCluster);  // the run's outputs are indexed by the old rows
   cudaStream_t st = h->stream;
-  const uint32_t N = h->n_pending, Rt = h->n_rr, M = h->n_ent;
-  const bool cp_pd = h->n_dead > 0, cp_rr = h->n_rr_dead > 0;
-  const uint32_t Nl = N - h->n_dead, Rl = Rt - h->n_rr_dead;
-  uint32_t gate_n = 0;  // rows of the new table with gate state: the live rows below gate_n
-  for (uint32_t r = 0; r < h->gate_n; ++r) gate_n += h->h_dead[r] ? 0 : 1;
+  const uint32_t N = h->pd.n, Rt = h->rr.n, M = h->ent.n;
+  const bool cp_pd = h->pd.n_dead > 0, cp_rr = h->rr.n_dead > 0;
+  const uint32_t Nl = N - h->pd.n_dead, Rl = Rt - h->rr.n_dead;
 
   // ---- work buffers, then the live rows, the maps and the open entries ----
   const size_t ns = std::max<size_t>({(size_t)N, (size_t)Rt, (size_t)M, 1});
@@ -1513,18 +1770,18 @@ int crane_sched_compact(crane_sched_t* h, uint32_t* pending_map, uint32_t* runni
   if (cp_pd) {
     CU(pd_live.ensure(std::max<uint32_t>(Nl, 1)));
     CU(pd_map.ensure(N));
-    TRY(live_rows(h, h->d_dead.p, N, Nl, pd_live.p, pd_map.p));
+    TRY(live_rows(h, h->pd.d_dead.p, N, Nl, pd_live.p, pd_map.p));
   }
   if (cp_rr) {
     CU(rr_live.ensure(std::max<uint32_t>(Rl, 1)));
     CU(rr_map.ensure(Rt));
-    TRY(live_rows(h, h->d_rr_dead.p, Rt, Rl, rr_live.p, rr_map.p));
+    TRY(live_rows(h, h->rr.d_dead.p, Rt, Rl, rr_live.p, rr_map.p));
   }
   uint32_t n_keep = 0;
   if (M) {
     CU(keep.ensure(M));
     CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
-    CRANE_LAUNCH(k_cp_ent_keys, (M + 255) / 256, 256, 0, st, gate_dev(h), h->n_dead ? h->d_dead.p : nullptr,
+    CRANE_LAUNCH(k_cp_ent_keys, (M + 255) / 256, 256, 0, st, gate_dev(h), h->pd.dead(),
                  h->d_keys_a.p, h->d_vals_a.p, h->d_flag.p);
     uint64_t* keys;
     uint32_t* vals;
@@ -1537,149 +1794,33 @@ int crane_sched_compact(crane_sched_t* h, uint32_t* pending_map, uint32_t* runni
   const bool cp_ent = M && (n_keep < M || cp_pd || cp_rr);
 
   // ---- every new buffer before the first gather: CRANE_ENOMEM leaves the tables as they were ----
-  std::vector<uint32_t> alloc_off, incl_off, excl_off, rr_alloc_off;
-  DBuf<uint32_t> partition, node_num, ntpn, ntpn_max, ntasks, part_prio, qos_prio, account, qos, user, pd_resv,
-      p_alloc_off, p_incl_off, p_incl_nodes, p_excl_off, p_excl_nodes, g_open;
-  DBuf<int64_t> time_limit, submit, g_begin;
-  DBuf<uint8_t> exclusive, dead, g_held, g_is_or;
-  DBuf<double> mandated;
-  DBuf<View> req_node, req_task, req_total;
-  DBuf<long long> g_ready;
-  if (cp_pd) {
-    const size_t n1 = std::max<uint32_t>(Nl, 1);
-    alloc_off = live_offsets(h->h_alloc_off, h->h_dead);
-    CU(partition.ensure(n1)); CU(time_limit.ensure(n1)); CU(submit.ensure(n1)); CU(node_num.ensure(n1));
-    CU(ntpn.ensure(n1)); CU(ntpn_max.ensure(n1)); CU(ntasks.ensure(n1)); CU(exclusive.ensure(n1));
-    CU(part_prio.ensure(n1)); CU(qos_prio.ensure(n1)); CU(account.ensure(n1));
-    CU(req_node.ensure(n1)); CU(req_task.ensure(n1)); CU(req_total.ensure(n1));
-    CU(dead.ensure(n1));
-    CU(p_alloc_off.ensure(n1 + 1));
-    if (h->have_qos_cols) { CU(qos.ensure(n1)); CU(user.ensure(n1)); }
-    if (h->have_mandated) CU(mandated.ensure(n1));
-    if (h->have_pd_resv) CU(pd_resv.ensure(n1));
-    if (h->have_lists_incl) {
-      incl_off = live_offsets(h->h_incl_off, h->h_dead);
-      CU(p_incl_off.ensure(n1 + 1));
-      CU(p_incl_nodes.ensure(std::max<uint32_t>(incl_off.back(), 1)));
-    }
-    if (h->have_lists_excl) {
-      excl_off = live_offsets(h->h_excl_off, h->h_dead);
-      CU(p_excl_off.ensure(n1 + 1));
-      CU(p_excl_nodes.ensure(std::max<uint32_t>(excl_off.back(), 1)));
-    }
-    if (h->gate_n) {
-      const size_t g1 = std::max<uint32_t>(gate_n, 1);
-      CU(g_held.ensure(g1)); CU(g_begin.ensure(g1)); CU(g_is_or.ensure(g1)); CU(g_open.ensure(g1)); CU(g_ready.ensure(g1));
-    }
-  }
-  DBuf<int64_t> rr_start, rr_end, rr_cpu;
-  DBuf<uint32_t> rr_node_num, rr_part_prio, rr_qos_prio, rr_account, rr_resv, r_alloc_off, rr_alloc_node;
-  DBuf<uint64_t> rr_mem;
-  DBuf<Row> rr_alloc_res;
-  DBuf<uint8_t> rr_dead;
-  if (cp_rr) {
-    const size_t r1 = std::max<uint32_t>(Rl, 1);
-    rr_alloc_off = live_offsets(h->h_rr_alloc_off, h->h_rr_dead);
-    CU(rr_start.ensure(r1)); CU(rr_end.ensure(r1)); CU(rr_cpu.ensure(r1)); CU(rr_node_num.ensure(r1));
-    CU(rr_part_prio.ensure(r1)); CU(rr_qos_prio.ensure(r1)); CU(rr_account.ensure(r1)); CU(rr_resv.ensure(r1));
-    CU(rr_mem.ensure(r1)); CU(rr_dead.ensure(r1));
-    CU(r_alloc_off.ensure(r1 + 1));
-    CU(rr_alloc_node.ensure(std::max<uint32_t>(rr_alloc_off.back(), 1)));
-    CU(rr_alloc_res.ensure(std::max<uint32_t>(rr_alloc_off.back(), 1)));
-  }
-  DBuf<uint32_t> e_dependent, e_dependee;
-  DBuf<uint8_t> e_kind, e_type, e_live;
-  DBuf<uint64_t> e_delay;
+  PendingTable pd;
+  GateRows gate;
+  RunningTable rr;
+  DepEntries ent;
+  if (cp_pd) TRY(pending_fresh(h, pd, gate));
+  if (cp_rr) TRY(running_fresh(h, rr));
   if (cp_ent) {
-    const size_t m1 = std::max<uint32_t>(n_keep, 1);
-    CU(e_dependent.ensure(m1)); CU(e_dependee.ensure(m1)); CU(e_kind.ensure(m1)); CU(e_type.ensure(m1));
-    CU(e_live.ensure(m1)); CU(e_delay.ensure(m1));
+    ent.n = n_keep;
+    CU(ensure_cols(ent, n_keep));
   }
 
   // ---- gathers ----
-  if (cp_pd) {
-    PendingCols s{h->d_partition.p, h->d_time_limit.p, h->d_submit.p, h->d_node_num.p, h->d_ntpn.p, h->d_ntpn_max.p,
-                  h->d_ntasks.p, h->d_exclusive.p, h->d_part_prio.p, h->d_qos_prio.p, h->d_account.p, h->d_qos.p,
-                  h->d_user.p, h->d_mandated.p, h->d_pd_resv.p, h->d_req_node.p, h->d_req_task.p, h->d_req_total.p,
-                  h->d_g_held.p, h->d_g_begin.p, h->d_g_is_or.p, h->d_g_open.p, h->d_g_ready.p};
-    PendingCols d{partition.p, time_limit.p, submit.p, node_num.p, ntpn.p, ntpn_max.p, ntasks.p, exclusive.p,
-                  part_prio.p, qos_prio.p, account.p, qos.p, user.p, mandated.p, pd_resv.p, req_node.p, req_task.p,
-                  req_total.p, g_held.p, g_begin.p, g_is_or.p, g_open.p, g_ready.p};
-    if (Nl) CRANE_LAUNCH(k_cp_pending, (Nl + 255) / 256, 256, 0, st, s, d, pd_live.p, Nl, gate_n);
-    CU(cudaMemsetAsync(dead.p, 0, std::max<uint32_t>(Nl, 1), st));
-    TRY(csr_offsets(h, h->d_alloc_off.p, pd_live.p, Nl, p_alloc_off.p));
-    if (h->have_lists_incl) {
-      TRY(csr_offsets(h, h->d_incl_off.p, pd_live.p, Nl, p_incl_off.p));
-      TRY(csr_copy(h, h->d_incl_off.p, h->d_incl_nodes.p, pd_live.p, Nl, p_incl_off.p, p_incl_nodes.p));
-    }
-    if (h->have_lists_excl) {
-      TRY(csr_offsets(h, h->d_excl_off.p, pd_live.p, Nl, p_excl_off.p));
-      TRY(csr_copy(h, h->d_excl_off.p, h->d_excl_nodes.p, pd_live.p, Nl, p_excl_off.p, p_excl_nodes.p));
-    }
-  }
-  if (cp_rr) {
-    const RunTableDev s = run_table(h);
-    RunTableDev d{};
-    d.start_time = rr_start.p; d.end_time = rr_end.p; d.node_num = rr_node_num.p; d.partition_priority = rr_part_prio.p;
-    d.qos_priority = rr_qos_prio.p; d.account = rr_account.p; d.reservation = rr_resv.p; d.view_cpu_raw = rr_cpu.p;
-    d.view_mem = rr_mem.p;
-    if (Rl) CRANE_LAUNCH(k_cp_running, (Rl + 255) / 256, 256, 0, st, s, d, rr_live.p, Rl);
-    CU(cudaMemsetAsync(rr_dead.p, 0, std::max<uint32_t>(Rl, 1), st));
-    TRY(csr_offsets(h, s.alloc_off, rr_live.p, Rl, r_alloc_off.p));
-    TRY(csr_copy(h, s.alloc_off, s.alloc_node, rr_live.p, Rl, r_alloc_off.p, rr_alloc_node.p));
-    TRY(csr_copy(h, s.alloc_off, s.alloc_res, rr_live.p, Rl, r_alloc_off.p, rr_alloc_res.p));
-  }
-  if (cp_ent && n_keep) {
-    GateDev d = gate_dev(h);
-    d.dependent = e_dependent.p; d.dependee = e_dependee.p; d.kind = e_kind.p; d.type = e_type.p; d.live = e_live.p;
-    CRANE_LAUNCH(k_cp_entries, (n_keep + 255) / 256, 256, 0, st, gate_dev(h), d, e_delay.p, keep.p, n_keep,
-                 cp_pd ? pd_map.p : nullptr, cp_rr ? rr_map.p : nullptr);
-  }
+  if (cp_pd) TRY(pending_copy(h, pd, gate, pd_live.p));
+  if (cp_rr) TRY(running_copy(h, rr, rr_live.p));
+  if (cp_ent && n_keep)
+    CRANE_LAUNCH(k_cp_entries, (n_keep + 255) / 256, 256, 0, st, gate_dev(h), gate_dev(gate, ent, nullptr), keep.p,
+                 n_keep, cp_pd ? pd_map.p : nullptr, cp_rr ? rr_map.p : nullptr);
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(st));
 
   // ---- the new tables replace the old ones (whose buffers go with the locals) ----
   if (cp_pd) {
-    h->d_partition.swap(partition); h->d_time_limit.swap(time_limit); h->d_submit.swap(submit);
-    h->d_node_num.swap(node_num); h->d_ntpn.swap(ntpn); h->d_ntpn_max.swap(ntpn_max); h->d_ntasks.swap(ntasks);
-    h->d_exclusive.swap(exclusive); h->d_part_prio.swap(part_prio); h->d_qos_prio.swap(qos_prio);
-    h->d_account.swap(account); h->d_req_node.swap(req_node); h->d_req_task.swap(req_task);
-    h->d_req_total.swap(req_total); h->d_dead.swap(dead); h->d_alloc_off.swap(p_alloc_off);
-    if (h->have_qos_cols) { h->d_qos.swap(qos); h->d_user.swap(user); }
-    if (h->have_mandated) h->d_mandated.swap(mandated);
-    if (h->have_pd_resv) h->d_pd_resv.swap(pd_resv);
-    if (h->have_lists_incl) { h->d_incl_off.swap(p_incl_off); h->d_incl_nodes.swap(p_incl_nodes); h->h_incl_off = incl_off; }
-    if (h->have_lists_excl) { h->d_excl_off.swap(p_excl_off); h->d_excl_nodes.swap(p_excl_nodes); h->h_excl_off = excl_off; }
-    if (h->gate_n) {
-      h->d_g_held.swap(g_held); h->d_g_begin.swap(g_begin); h->d_g_is_or.swap(g_is_or); h->d_g_open.swap(g_open);
-      h->d_g_ready.swap(g_ready);
-      h->h_has_deps = live_only(h->h_has_deps, std::vector<uint8_t>(h->h_dead.begin(), h->h_dead.begin() + h->gate_n));
-    }
-    h->h_alloc_off = alloc_off;
-    h->h_pd_account = live_only(h->h_pd_account, h->h_dead);
-    h->h_dead.assign(Nl, 0);
-    h->n_dead = 0;
-    h->n_pending = Nl;
-    h->total_alloc = alloc_off.back();
-    h->gate_n = gate_n;
+    std::swap(h->pd, pd);
+    std::swap(h->gate, gate);
   }
-  if (cp_rr) {
-    h->d_rr_start.swap(rr_start); h->d_rr_end.swap(rr_end); h->d_rr_cpu.swap(rr_cpu); h->d_rr_node_num.swap(rr_node_num);
-    h->d_rr_part_prio.swap(rr_part_prio); h->d_rr_qos_prio.swap(rr_qos_prio); h->d_rr_account.swap(rr_account);
-    h->d_rr_resv.swap(rr_resv); h->d_rr_mem.swap(rr_mem); h->d_rr_dead.swap(rr_dead);
-    h->d_rr_alloc_off.swap(r_alloc_off); h->d_rr_alloc_node.swap(rr_alloc_node); h->d_rr_alloc_res.swap(rr_alloc_res);
-    h->h_rr_account = live_only(h->h_rr_account, h->h_rr_dead);
-    h->h_rr_alloc_off = rr_alloc_off;
-    h->h_rr_dead.assign(Rl, 0);
-    h->n_rr_dead = 0;
-    h->n_rr = Rl;
-    // (the run's view of the running table is the live rows in row order: rr_dirty stays)
-  }
-  if (cp_ent) {
-    h->d_e_dependent.swap(e_dependent); h->d_e_dependee.swap(e_dependee); h->d_e_kind.swap(e_kind);
-    h->d_e_type.swap(e_type); h->d_e_live.swap(e_live); h->d_e_delay.swap(e_delay);
-    h->n_ent = n_keep;
-  }
+  if (cp_rr) std::swap(h->rr, rr);
+  if (cp_ent) std::swap(h->ent, ent);
   if (cp_pd || cp_rr) {
     // work and output buffers sized for the old tables: keep_running sizes them again
     h->d_keys_a.release(); h->d_keys_b.release(); h->d_vals_a.release(); h->d_vals_b.release();
@@ -1749,44 +1890,21 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
   lower_stage(h, kUploaded);  // the previous run's outputs are void from here on
   (void)cudaGetLastError();  // a stale error of an earlier, unrelated call in this process is not this run's
   cudaStream_t st = h->stream;
-  const uint32_t N = h->n_pending, R = h->n_running;
+  const uint32_t N = h->pd.n, R = h->n_running;
   h->timing.kernel_launches = 0;
 
-  PendingDev pd{};
-  pd.n = N;
-  pd.partition = h->d_partition.p;
-  pd.time_limit = h->d_time_limit.p;
-  pd.submit_time = h->d_submit.p;
-  pd.node_num = h->d_node_num.p;
-  pd.ntasks_per_node_min = h->d_ntpn.p;
-  pd.ntasks_per_node_max = h->d_ntpn_max.p;
-  pd.ntasks = h->d_ntasks.p;
-  pd.exclusive = h->d_exclusive.p;
-  pd.partition_priority = h->d_part_prio.p;
-  pd.qos_priority = h->d_qos_prio.p;
-  pd.account = h->d_account.p;
-  pd.mandated_priority = h->have_mandated ? h->d_mandated.p : nullptr;
-  pd.req_node = h->d_req_node.p;
-  pd.req_task = h->d_req_task.p;
-  pd.req_total = h->d_req_total.p;
-  pd.incl_off = h->have_lists_incl ? h->d_incl_off.p : nullptr;
-  pd.incl_nodes = h->d_incl_nodes.p;
-  pd.excl_off = h->have_lists_excl ? h->d_excl_off.p : nullptr;
-  pd.excl_nodes = h->d_excl_nodes.p;
-  pd.alloc_off = h->d_alloc_off.p;
-  pd.reservation = h->have_pd_resv ? h->d_pd_resv.p : nullptr;
-  pd.dead = h->n_dead ? h->d_dead.p : nullptr;
+  PendingDev pd = h->pd.dev();
 
   RunningDev rn{};
   rn.n = R;
-  rn.start_time = h->d_rn_start.p;
-  rn.end_time = h->d_rn_end.p;
-  rn.node_num = h->d_rn_node_num.p;
-  rn.partition_priority = h->d_rn_part_prio.p;
-  rn.qos_priority = h->d_rn_qos_prio.p;
-  rn.account = h->d_rn_account.p;
-  rn.view_cpu_raw = h->d_rn_cpu.p;
-  rn.view_mem = h->d_rn_mem.p;
+  rn.start_time = h->rn.d_rr_start.p;
+  rn.end_time = h->rn.d_rr_end.p;
+  rn.node_num = h->rn.d_rr_node_num.p;
+  rn.partition_priority = h->rn.d_rr_part_prio.p;
+  rn.qos_priority = h->rn.d_rr_qos_prio.p;
+  rn.account = h->rn.d_rr_account.p;
+  rn.view_cpu_raw = h->rn.d_rr_cpu.p;
+  rn.view_mem = h->rn.d_rr_mem.p;
   rn.slot_off = h->d_rn_slot_off.p;
   rn.slot_end = h->d_rn_slot_end.p;
   rn.slot_res = h->d_rn_slot_res.p;
@@ -1839,10 +1957,10 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
 
   // ---- node state / timelines (R2,R3,R4) -----------------------------------
   CU(cudaEventRecord(h->ev[kEvRunBegin], st));
-  if (h->total_alloc) {  // allocation slots of jobs without a placement read as zero
-    CU(cudaMemsetAsync(h->d_out_node.p, 0, sizeof(uint32_t) * h->total_alloc, st));
-    CU(cudaMemsetAsync(h->d_out_ntasks.p, 0, sizeof(uint32_t) * h->total_alloc, st));
-    CU(cudaMemsetAsync(h->d_out_res.p, 0, sizeof(Row) * h->total_alloc, st));
+  if (h->pd.total_alloc) {  // allocation slots of jobs without a placement read as zero
+    CU(cudaMemsetAsync(h->d_out_node.p, 0, sizeof(uint32_t) * h->pd.total_alloc, st));
+    CU(cudaMemsetAsync(h->d_out_ntasks.p, 0, sizeof(uint32_t) * h->pd.total_alloc, st));
+    CU(cudaMemsetAsync(h->d_out_res.p, 0, sizeof(Row) * h->pd.total_alloc, st));
   }
   if (h->n_slots) {
     CRANE_LAUNCH(k_node_init, (h->n_slots + 127) / 128, 128, 0, st, cl, rn, tl, now, h->cfg.max_jobs_per_node, h->cfg.cost_policy);
@@ -1851,7 +1969,7 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
   CU(cudaEventRecord(h->ev[kEvInitEnd], st));
 
   // ---- the gate: held, not-yet-begun and dependent rows sit this run out ----
-  const bool gated = h->gate_on && N;
+  const bool gated = h->gate.on && N;
   if (gated) {
     TRY(gate_fit(h));
     CU(h->d_g_code.ensure(N));
@@ -1861,8 +1979,8 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     // an account with only gated rows does not seed the fair-share bounds
     if (h->n_accounts) {
       CU(cudaMemsetAsync(h->d_acc_present.p, 0, h->n_accounts, st));
-      CRANE_LAUNCH(k_acc_present, (N + R + 255) / 256, 256, 0, st, h->d_account.p, h->d_g_code.p, N,
-                   h->d_rn_account.p, R, h->d_acc_present.p);
+      CRANE_LAUNCH(k_acc_present, (N + R + 255) / 256, 256, 0, st, h->pd.d_account.p, h->d_g_code.p, N,
+                   h->rn.d_rr_account.p, R, h->d_acc_present.p);
       h->timing.kernel_launches++;
     }
   }
@@ -1897,7 +2015,7 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     CRANE_LAUNCH(k_priority, (N + 255) / 256, 256, 0, st, pd, pc, now, h->d_bounds.p, h->d_acc_service.p,
                  h->d_prio.p, h->d_keys_a.p, h->d_vals_a.p);
     h->timing.kernel_launches++;
-    if (pc.type != 0 || h->n_dead || gated)  // (FIFO keeps input order; excluded rows only have to go behind the others)
+    if (pc.type != 0 || h->pd.n_dead || gated)  // (FIFO keeps input order; excluded rows only have to go behind the others)
       TRY(radix_sort(h, N, pc.type != 0 ? 64 : 8, &keys, &vals));
     // keys2 go to the buffer not holding `vals`
     uint64_t* key2 = h->d_keys_a.p;
@@ -1951,8 +2069,8 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     c2.sched_nparts = h->max_comp_parts > 1 ? h->d_sched_nparts.p : nullptr;
     c2.slot_memb = h->d_slot_memb.p;
     c2.dslot = (uint32_t)h->dict_slot;
-    c2.req_node = h->d_req_node.p;
-    c2.req_task = h->d_req_task.p;
+    c2.req_node = h->pd.d_req_node.p;
+    c2.req_task = h->pd.d_req_task.p;
     size_t smem = commit2_smem_bytes(h->max_part_slots, h->words_per_row, c2.gres != 0, h->v2_ring, h->max_comp_parts);
     uint32_t grid = h->n_vparts;
     if (h->shard_n > 1) {
@@ -1977,10 +2095,10 @@ int crane_sched_fetch(crane_sched_t* h, crane_placements_t* out) {
   TRY(require(h, kRan, "fetch"));
   CU(cudaSetDevice(h->device));
   cudaStream_t st = h->stream;
-  const uint32_t N = h->n_pending;
+  const uint32_t N = h->pd.n;
   if (N && (!out->reason || !out->priority || !out->start_time || !out->end_time || !out->n_alloc || !out->alloc_off))
     return fail(h, CRANE_EINVAL, "placements: null column");
-  if (h->total_alloc && (!out->alloc_node || !out->alloc_ntasks || !out->alloc_res))
+  if (h->pd.total_alloc && (!out->alloc_node || !out->alloc_ntasks || !out->alloc_res))
     return fail(h, CRANE_EINVAL, "placements: null allocation table");
   // slots of jobs without a placement stay zero
   if (N) {
@@ -1990,12 +2108,12 @@ int crane_sched_fetch(crane_sched_t* h, crane_placements_t* out) {
     CU(cudaMemcpyAsync(out->end_time, h->d_out_end.p, sizeof(int64_t) * N, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(out->n_alloc, h->d_out_nalloc.p, sizeof(uint32_t) * N, cudaMemcpyDeviceToHost, st));
   }
-  if (h->total_alloc) {
-    CU(cudaMemcpyAsync(out->alloc_node, h->d_out_node.p, sizeof(uint32_t) * h->total_alloc, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(out->alloc_ntasks, h->d_out_ntasks.p, sizeof(uint32_t) * h->total_alloc, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(out->alloc_res, h->d_out_res.p, sizeof(Row) * h->total_alloc, cudaMemcpyDeviceToHost, st));
+  if (h->pd.total_alloc) {
+    CU(cudaMemcpyAsync(out->alloc_node, h->d_out_node.p, sizeof(uint32_t) * h->pd.total_alloc, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->alloc_ntasks, h->d_out_ntasks.p, sizeof(uint32_t) * h->pd.total_alloc, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->alloc_res, h->d_out_res.p, sizeof(Row) * h->pd.total_alloc, cudaMemcpyDeviceToHost, st));
   }
-  memcpy(out->alloc_off, h->h_alloc_off.data(), sizeof(uint32_t) * ((size_t)N + 1));
+  memcpy(out->alloc_off, h->pd.h_alloc_off.data(), sizeof(uint32_t) * ((size_t)N + 1));
   CU(cudaEventRecord(h->ev[kEvD2hEnd], st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
@@ -2036,9 +2154,9 @@ int crane_sched_debug_profile(crane_sched_t* h, unsigned long long* dst, size_t 
 int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_t* reason) {
   if (!h || !qt || !reason) return CRANE_EINVAL;
   TRY(require(h, kRan, "qos_filter"));
-  if (!h->have_qos_cols) return fail(h, CRANE_EINVAL, "qos_filter: pending.qos / pending.user were not uploaded");
+  if (!h->pd.have_qos_cols) return fail(h, CRANE_EINVAL, "qos_filter: pending.qos / pending.user were not uploaded");
   CU(cudaSetDevice(h->device));
-  const uint32_t N = h->n_pending, Q = qt->n_qos, U = qt->n_users, A = qt->n_accounts;
+  const uint32_t N = h->pd.n, Q = qt->n_qos, U = qt->n_users, A = qt->n_accounts;
   if (Q == 0 || Q >= 65535) return fail(h, CRANE_EINVAL, "qos_filter: n_qos out of range");
   if (A > 65535) return fail(h, CRANE_ENOSYS, "qos_filter: more than 65535 accounts");
   if (!qt->valid || !qt->max_jobs_per_user || !qt->max_jobs_per_account || !qt->max_jobs ||
@@ -2062,7 +2180,7 @@ int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_
   // (pending.user was validated only for presence at upload)
   {
     std::vector<uint32_t> users(N);
-    if (N) CU(cudaMemcpyAsync(users.data(), h->d_user.p, (size_t)N * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (N) CU(cudaMemcpyAsync(users.data(), h->pd.d_user.p, (size_t)N * 4, cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     for (uint32_t i = 0; i < N; ++i)
       if (users[i] >= U) return fail(h, CRANE_EINVAL, "qos_filter: pending[%u]: user out of range", i);
@@ -2092,8 +2210,8 @@ int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_
   q.tres_user = h->d_q_tres.p; q.tres_account = h->d_q_tres.p + Q; q.tres_qos = h->d_q_tres.p + 2 * Q;
   q.chain_off = h->d_q_chain_off.p; q.chain_acct = h->d_q_chain.p;
   q.user_usage = h->d_q_user_usage.p; q.account_usage = h->d_q_acct_usage.p; q.qos_usage = h->d_q_qos_usage.p;
-  q.qos = h->d_qos.p; q.user = h->d_user.p; q.time_limit = h->d_time_limit.p;
-  q.n_alloc = h->d_out_nalloc.p; q.alloc_off = h->d_alloc_off.p; q.alloc_res = h->d_out_res.p;
+  q.qos = h->pd.d_qos.p; q.user = h->pd.d_user.p; q.time_limit = h->pd.d_time_limit.p;
+  q.n_alloc = h->d_out_nalloc.p; q.alloc_off = h->pd.d_alloc_off.p; q.alloc_res = h->d_out_res.p;
   q.reason = h->d_reason.p;
   if (N) {
     // the jobs the pass walks, grouped by qos in job-id order: key + stable radix sort
@@ -2220,76 +2338,6 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
   return CRANE_OK;
 }
 
-}  // extern "C"
-
-// ---- the step state of running jobs, resident on the device -------------------------
-namespace {
-
-enum : uint8_t { kSpPending = 0, kSpScheduled = 1, kSpErased = 2 };
-
-void sj_dirty(crane_sched* h, uint32_t j) {
-  if (!h->h_sj_dirty[j]) {
-    h->h_sj_dirty[j] = 1;
-    h->h_sj_dirty_rows.push_back(j);
-  }
-}
-
-// The rows of an erase / start / read call: in [0, n_rows), not erased, none listed twice
-template <class Erased>
-int check_rows(crane_sched* h, const char* call, const uint32_t* rows, uint32_t n, uint32_t n_rows, Erased erased) {
-  if (n && !rows) return fail(h, CRANE_EINVAL, "%s: null rows", call);
-  std::vector<uint32_t> sorted(rows, rows + n);
-  std::sort(sorted.begin(), sorted.end());
-  for (uint32_t k = 0; k < n; ++k) {
-    if (sorted[k] >= n_rows) return fail(h, CRANE_EINVAL, "%s: row %u out of range", call, sorted[k]);
-    if (erased(sorted[k])) return fail(h, CRANE_EINVAL, "%s: row %u was erased", call, sorted[k]);
-    if (k && sorted[k] == sorted[k - 1]) return fail(h, CRANE_EINVAL, "%s: row %u listed twice", call, sorted[k]);
-  }
-  return CRANE_OK;
-}
-
-// New step-job rows whose nodes and avail are in the pools up to off.back()
-void sj_commit(crane_sched* h, const std::vector<uint32_t>& off) {
-  for (size_t k = 0; k + 1 < off.size(); ++k) {
-    h->h_sj_node_off.push_back(off[k + 1]);
-    h->h_sj_dead.push_back(0);
-    h->h_sj_dirty.push_back(0);
-    h->h_sj_queue.emplace_back();
-    sj_dirty(h, h->n_sj++);
-  }
-}
-
-StepPoolDev step_pool(crane_sched* h) {
-  StepPoolDev p{};
-  p.sj_node_off = h->d_sj_node_off.p;
-  p.sj_node = h->d_sj_node.p;
-  p.sj_avail = h->d_sj_avail.p;
-  p.job = h->d_sp_job.p;
-  p.node_num = h->d_sp_nn.p;
-  p.ntasks = h->d_sp_nt.p;
-  p.ntpn_min = h->d_sp_t0.p;
-  p.ntpn_max = h->d_sp_t1.p;
-  p.req_node = h->d_sp_req_node.p;
-  p.req_task = h->d_sp_req_task.p;
-  p.incl_off = h->d_sp_incl_off.p;
-  p.incl_nodes = h->d_sp_incl.p;
-  p.excl_off = h->d_sp_excl_off.p;
-  p.excl_nodes = h->d_sp_excl.p;
-  p.alloc_at = h->d_sp_alloc_at.p;
-  p.sa_node = h->d_sa_node.p;
-  p.sa_res = h->d_sa_res.p;
-  return p;
-}
-
-// grid of a kernel with one warp per item, 256 threads per block
-uint32_t warp_grid(const crane_sched* h, uint64_t items) {
-  return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((items + 7) / 8, 8ull * h->n_sm));
-}
-
-}  // namespace
-
-extern "C" {
-
 int crane_sched_step_jobs_reset(crane_sched_t* h) {
   if (!h) return CRANE_EINVAL;
   TRY(require(h, kCluster, "step_jobs_reset"));
@@ -2312,14 +2360,14 @@ int crane_sched_step_jobs_reset(crane_sched_t* h) {
 int crane_sched_step_jobs_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32_t* first) {
   if (!h) return CRANE_EINVAL;
   TRY(require(h, kCluster, "step_jobs_start"));
-  TRY(check_rows(h, "step_jobs_start", rows, n, h->n_rr, [&](uint32_t r) { return h->h_rr_dead[r] != 0; }));
+  TRY(check_rows(h, "step_jobs_start", rows, n, h->rr.n, [&](uint32_t r) { return h->rr.h_dead[r] != 0; }));
   CU(cudaSetDevice(h->device));
   h->sp_results = false;
   cudaStream_t st = h->stream;
   const uint32_t base = h->n_sj, eb = h->h_sj_node_off.back();
   std::vector<uint32_t> off(n + 1, eb);
   for (uint32_t k = 0; k < n; ++k) {
-    const uint64_t e = (uint64_t)off[k] + (h->h_rr_alloc_off[rows[k] + 1] - h->h_rr_alloc_off[rows[k]]);
+    const uint64_t e = (uint64_t)off[k] + (h->rr.h_rr_alloc_off[rows[k] + 1] - h->rr.h_rr_alloc_off[rows[k]]);
     if (e > 0xfffffff0ull || (uint64_t)base + n > 0xfffffff0ull) return fail(h, CRANE_EINVAL, "step_jobs_start: too many rows");
     off[k + 1] = (uint32_t)e;
   }
@@ -2330,7 +2378,7 @@ int crane_sched_step_jobs_start(crane_sched_t* h, const uint32_t* rows, uint32_t
     H2D(h->d_sp_call, rows, n);
     CU(h->d_sp_flag.ensure(1));
     CU(cudaMemsetAsync(h->d_sp_flag.p, 0, sizeof(uint32_t), st));
-    CRANE_LAUNCH(k_sj_seed, warp_grid(h, n), 256, 0, st, h->d_rr_alloc_off.p, h->d_rr_alloc_node.p, h->d_rr_alloc_res.p,
+    CRANE_LAUNCH(k_sj_seed, warp_grid(h, n), 256, 0, st, h->rr.d_rr_alloc_off.p, h->rr.d_rr_alloc_node.p, h->rr.d_rr_alloc_res.p,
                  h->d_sp_call.p, n, h->d_sj_node_off.p + base, h->d_sj_node.p, h->d_sj_avail.p, h->d_sp_flag.p);
     uint32_t bad = 0;
     CU(cudaMemcpyAsync(&bad, h->d_sp_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
