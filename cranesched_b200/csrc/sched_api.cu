@@ -343,6 +343,110 @@ struct RunningTable : Tombstones, RunCols {
   }
 };
 
+// The resident step jobs (crane_sched_step_jobs_start, _append): each job's nodes and
+// one avail row per node, in a node pool. Rows keep their index; an erased row has no
+// device tombstone, since every kernel reaches the rows through lists the host builds.
+struct StepJobTable {
+  uint32_t n = 0;
+  // host mirrors
+  std::vector<uint32_t> h_node_off = {0};      // [n + 1]
+  std::vector<uint8_t> h_dead, h_dirty;
+  std::vector<uint32_t> h_dirty_rows;          // the rows with h_dirty set
+  std::vector<std::vector<uint32_t>> h_queue;  // live pending step rows of each job, row order
+  DBuf<uint32_t> d_node_off, d_node;
+  DBuf<Row> d_avail;
+
+  void mark_dirty(uint32_t j) {
+    if (!h_dirty[j]) {
+      h_dirty[j] = 1;
+      h_dirty_rows.push_back(j);
+    }
+  }
+
+  // New rows whose nodes and avail are in the pool up to off.back()
+  void commit(const std::vector<uint32_t>& off) {
+    for (size_t k = 0; k + 1 < off.size(); ++k) {
+      h_node_off.push_back(off[k + 1]);
+      h_dead.push_back(0);
+      h_dirty.push_back(0);
+      h_queue.emplace_back();
+      mark_dirty(n++);
+    }
+  }
+
+  void reset() {
+    n = 0;
+    h_node_off.assign(1, 0);
+    h_dead.clear();
+    h_dirty.clear();
+    h_dirty_rows.clear();
+    h_queue.clear();
+  }
+};
+
+enum : uint8_t { kSpPending = 0, kSpScheduled = 1, kSpErased = 2 };
+
+// The resident steps (crane_sched_steps_append), and the allocation pool that holds the
+// node rows of the scheduled ones
+struct StepTable {
+  uint32_t n = 0, n_alloc = 0;  // step rows, allocation-pool rows
+  // host mirrors
+  std::vector<uint32_t> h_job, h_nn, h_nt, h_incl_off = {0}, h_excl_off = {0};
+  std::vector<uint8_t> h_state;  // kSpPending, kSpScheduled, kSpErased
+  DBuf<uint32_t> d_job, d_nn, d_nt, d_t0, d_t1, d_incl_off, d_incl, d_excl_off, d_excl, d_alloc_at;
+  DBuf<View> d_req_node, d_req_task;
+  DBuf<uint32_t> d_sa_node;
+  DBuf<Row> d_sa_res;
+
+  void reset() {
+    n = n_alloc = 0;
+    h_job.clear();
+    h_nn.clear();
+    h_nt.clear();
+    h_state.clear();
+    h_incl_off.assign(1, 0);
+    h_excl_off.assign(1, 0);
+  }
+};
+
+StepPoolDev step_pool(const StepJobTable& sj, const StepTable& sp) {
+  StepPoolDev p{};
+  p.sj_node_off = sj.d_node_off.p;
+  p.sj_node = sj.d_node.p;
+  p.sj_avail = sj.d_avail.p;
+  p.job = sp.d_job.p;
+  p.node_num = sp.d_nn.p;
+  p.ntasks = sp.d_nt.p;
+  p.ntpn_min = sp.d_t0.p;
+  p.ntpn_max = sp.d_t1.p;
+  p.req_node = sp.d_req_node.p;
+  p.req_task = sp.d_req_task.p;
+  p.incl_off = sp.d_incl_off.p;
+  p.incl_nodes = sp.d_incl.p;
+  p.excl_off = sp.d_excl_off.p;
+  p.excl_nodes = sp.d_excl.p;
+  p.alloc_at = sp.d_alloc_at.p;
+  p.sa_node = sp.d_sa_node.p;
+  p.sa_res = sp.d_sa_res.p;
+  return p;
+}
+
+// The results of the last steps_run: its scheduled steps in ascending row order
+struct StepResults {
+  bool valid = false;    // steps_fetch may be called
+  uint32_t sa_base = 0;  // their node rows start here in the allocation pool
+  std::vector<uint32_t> h_rows, h_node_off, h_task_off;
+  DBuf<uint32_t> d_u32;  // ntasks | task_node
+  DBuf<Row> d_rows;      // task_res
+
+  void clear() {
+    valid = false;
+    h_rows.clear();
+    h_node_off.assign(1, 0);
+    h_task_off.assign(1, 0);
+  }
+};
+
 // How far a handle has got; each stage needs every earlier one. A call that replaces
 // the tables of a stage lowers the handle to the stage before it.
 enum Stage { kNone, kCluster, kUploaded, kRan };
@@ -452,35 +556,17 @@ struct crane_sched {
   DBuf<uint8_t> d_q_valid;
   DBuf<crane_tres_limit_t> d_q_tres;
   DBuf<crane_meta_resource_t> d_q_user_usage, d_q_acct_usage, d_q_qos_usage;
-  // step scheduler (per call)
-  DBuf<uint32_t> d_st_u32;   // job node_off | node | step_off | step columns | lists | out offsets | placed | alloc_node | alloc_ntasks | task_node
-  DBuf<Row> d_st_rows;       // avail | alloc_res | task_res
-  DBuf<View> d_st_views;     // req_node | req_task
-  DBuf<uint8_t> d_st_sched;
-  // resident step state (step_resident_kernels.cuh): host mirrors of the small columns
-  uint32_t n_sj = 0, n_sp = 0, n_sa = 0;        // step-job rows, step rows, allocation-pool rows
-  std::vector<uint32_t> h_sj_node_off = {0};    // [n_sj + 1]
-  std::vector<uint8_t> h_sj_dead, h_sj_dirty;
-  std::vector<std::vector<uint32_t>> h_sj_queue;  // live pending step rows of each job, row order
-  std::vector<uint32_t> h_sj_dirty_rows;        // the rows with h_sj_dirty set
-  std::vector<uint32_t> h_sp_job, h_sp_nn, h_sp_nt, h_sp_incl_off = {0}, h_sp_excl_off = {0};
-  std::vector<uint8_t> h_sp_state;              // kSpPending, kSpScheduled, kSpErased
-  DBuf<uint32_t> d_sj_node_off, d_sj_node;
-  DBuf<Row> d_sj_avail;
-  DBuf<uint32_t> d_sp_job, d_sp_nn, d_sp_nt, d_sp_t0, d_sp_t1, d_sp_incl_off, d_sp_incl, d_sp_excl_off, d_sp_excl,
-      d_sp_alloc_at;
-  DBuf<View> d_sp_req_node, d_sp_req_task;
-  DBuf<uint32_t> d_sa_node;
-  DBuf<Row> d_sa_res;
-  // the last pass: the dense tables, its results and what the host knows of them
-  DBuf<uint32_t> d_sq_u32, d_sr_u32;            // dense u32 columns | results: ntasks, task_node
-  DBuf<Row> d_sq_rows, d_sr_rows;               // dense avail, alloc_res, task_res | results: task_res
-  DBuf<View> d_sq_views;
-  DBuf<uint8_t> d_sq_sched;
-  DBuf<uint32_t> d_sp_call, d_sp_flag;          // per call: rows and offsets | the seed's check
-  bool sp_results = false;                      // steps_fetch may be called
-  uint32_t sr_sa_base = 0;
-  std::vector<uint32_t> h_sr_rows, h_sr_node_off, h_sr_task_off;
+  // the resident step state (step_resident_kernels.cuh)
+  StepJobTable sj;
+  StepTable sp;
+  StepResults sr;
+  // per call, nothing in them outlives the call: the dense tables of a k_steps launch (u32 columns |
+  // avail, alloc_res, task_res | req_node, req_task | scheduled), each entry point with its own layout
+  DBuf<uint32_t> d_steps_u32;
+  DBuf<Row> d_steps_rows;
+  DBuf<View> d_steps_views;
+  DBuf<uint8_t> d_steps_sched;
+  DBuf<uint32_t> d_sp_call;  // per call: rows and offsets
 
   // the buffers free themselves after this, on the handle's device
   ~crane_sched() {
@@ -1277,48 +1363,27 @@ int running_copy(crane_sched* h, RunningTable& rr, const uint32_t* live) {
   return CRANE_OK;
 }
 
-// ---- the step state of running jobs, resident on the device -------------------------
+// ---- the step scheduler --------------------------------------------------------------
 
-enum : uint8_t { kSpPending = 0, kSpScheduled = 1, kSpErased = 2 };
-
-void sj_dirty(crane_sched* h, uint32_t j) {
-  if (!h->h_sj_dirty[j]) {
-    h->h_sj_dirty[j] = 1;
-    h->h_sj_dirty_rows.push_back(j);
-  }
+// The nodes of a host step-job table (crane_sched_schedule_steps, crane_sched_step_jobs_append):
+// its node_off, and each job's nodes in range, ascending and distinct
+int check_step_jobs(crane_sched* h, const crane_step_jobs_t* jb) {
+  const uint32_t J = jb->n_jobs;
+  TRY(check_offsets(h, "step jobs: node_off", jb->node_off, J));
+  if (jb->node_off[J] && (!jb->node || !jb->avail)) return fail(h, CRANE_EINVAL, "step jobs: null node table");
+  for (uint32_t j = 0; j < J; ++j)
+    for (uint32_t k = jb->node_off[j]; k < jb->node_off[j + 1]; ++k) {
+      if (jb->node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "step jobs[%u]: node %u out of range", j, jb->node[k]);
+      if (k > jb->node_off[j] && jb->node[k] <= jb->node[k - 1])
+        return fail(h, CRANE_EINVAL, "step jobs[%u]: nodes must be ascending and distinct", j);
+    }
+  return CRANE_OK;
 }
 
-// New step-job rows whose nodes and avail are in the pools up to off.back()
-void sj_commit(crane_sched* h, const std::vector<uint32_t>& off) {
-  for (size_t k = 0; k + 1 < off.size(); ++k) {
-    h->h_sj_node_off.push_back(off[k + 1]);
-    h->h_sj_dead.push_back(0);
-    h->h_sj_dirty.push_back(0);
-    h->h_sj_queue.emplace_back();
-    sj_dirty(h, h->n_sj++);
-  }
-}
-
-StepPoolDev step_pool(crane_sched* h) {
-  StepPoolDev p{};
-  p.sj_node_off = h->d_sj_node_off.p;
-  p.sj_node = h->d_sj_node.p;
-  p.sj_avail = h->d_sj_avail.p;
-  p.job = h->d_sp_job.p;
-  p.node_num = h->d_sp_nn.p;
-  p.ntasks = h->d_sp_nt.p;
-  p.ntpn_min = h->d_sp_t0.p;
-  p.ntpn_max = h->d_sp_t1.p;
-  p.req_node = h->d_sp_req_node.p;
-  p.req_task = h->d_sp_req_task.p;
-  p.incl_off = h->d_sp_incl_off.p;
-  p.incl_nodes = h->d_sp_incl.p;
-  p.excl_off = h->d_sp_excl_off.p;
-  p.excl_nodes = h->d_sp_excl.p;
-  p.alloc_at = h->d_sp_alloc_at.p;
-  p.sa_node = h->d_sa_node.p;
-  p.sa_res = h->d_sa_res.p;
-  return p;
+// k_steps over the jobs of dj, one warp per job
+void launch_steps(crane_sched* h, const StepJobsDev& dj, const StepsDev& ds, const StepOutDev& dout) {
+  const uint32_t grid = std::min<uint32_t>((dj.n_jobs + kStepWarps - 1) / kStepWarps, 16 * h->n_sm);
+  CRANE_LAUNCH(k_steps, grid, 32 * kStepWarps, 0, h->stream, dj, ds, dout, (uint32_t)h->dict_slot);
 }
 
 // grid of a kernel with one warp per item, 256 threads per block
@@ -2250,17 +2315,10 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
   if (!h || !jb || !st || !out) return CRANE_EINVAL;
   TRY(require(h, kCluster, "schedule_steps"));
   const uint32_t J = jb->n_jobs;
-  TRY(check_offsets(h, "step jobs: node_off", jb->node_off, J));
+  TRY(check_step_jobs(h, jb));
   TRY(check_offsets(h, "step jobs: step_off", jb->step_off, J));
   const uint32_t E = jb->node_off[J], S = jb->step_off[J];
   if (st->n != S) return fail(h, CRANE_EINVAL, "steps: n (%u) != step_off[n_jobs] (%u)", st->n, S);
-  if (E && (!jb->node || !jb->avail)) return fail(h, CRANE_EINVAL, "step jobs: null node table");
-  for (uint32_t j = 0; j < J; ++j)
-    for (uint32_t k = jb->node_off[j]; k < jb->node_off[j + 1]; ++k) {
-      if (jb->node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "step jobs[%u]: node %u out of range", j, jb->node[k]);
-      if (k > jb->node_off[j] && jb->node[k] <= jb->node[k - 1])
-        return fail(h, CRANE_EINVAL, "step jobs[%u]: nodes must be ascending and distinct", j);
-    }
   uint64_t nrows = 0, trows = 0;
   TRY(check_steps(h, st, &nrows, &trows));
   if ((J && !out->placed) || (S && (!out->scheduled || !out->node_off || !out->task_off)) || !out->node_off || !out->task_off ||
@@ -2292,13 +2350,13 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
   const size_t n_in = u.size();
   const size_t o_placed = n_in, o_anode = o_placed + J, o_antasks = o_anode + nrows, o_tnode = o_antasks + nrows;
   const size_t n_u32 = o_tnode + trows;
-  CU(h->d_st_u32.ensure(std::max<size_t>(n_u32, 1)));
-  CU(h->d_st_rows.ensure(std::max<size_t>(E + nrows + trows, 1)));
-  CU(h->d_st_views.ensure(std::max<size_t>(2 * (size_t)S, 1)));
-  CU(h->d_st_sched.ensure(std::max<size_t>(S, 1)));
-  uint32_t* du = h->d_st_u32.p;
-  Row* dr = h->d_st_rows.p;
-  View* dv = h->d_st_views.p;
+  CU(h->d_steps_u32.ensure(std::max<size_t>(n_u32, 1)));
+  CU(h->d_steps_rows.ensure(std::max<size_t>(E + nrows + trows, 1)));
+  CU(h->d_steps_views.ensure(std::max<size_t>(2 * (size_t)S, 1)));
+  CU(h->d_steps_sched.ensure(std::max<size_t>(S, 1)));
+  uint32_t* du = h->d_steps_u32.p;
+  Row* dr = h->d_steps_rows.p;
+  View* dv = h->d_steps_views.p;
   CU(cudaMemcpyAsync(du, u.data(), n_in * sizeof(uint32_t), cudaMemcpyHostToDevice, sm));
   if (n_u32 > n_in) CU(cudaMemsetAsync(du + n_in, 0, (n_u32 - n_in) * sizeof(uint32_t), sm));
   if (E) CU(cudaMemcpyAsync(dr, jb->avail, E * sizeof(Row), cudaMemcpyHostToDevice, sm));
@@ -2306,22 +2364,21 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
   if (S) {
     CU(cudaMemcpyAsync(dv, st->req_node, S * sizeof(View), cudaMemcpyHostToDevice, sm));
     CU(cudaMemcpyAsync(dv + S, st->req_task, S * sizeof(View), cudaMemcpyHostToDevice, sm));
-    CU(cudaMemsetAsync(h->d_st_sched.p, 0, S, sm));
+    CU(cudaMemsetAsync(h->d_steps_sched.p, 0, S, sm));
   }
   StepJobsDev dj{J, du + o_noff, du + o_node, dr, du + o_soff};
   StepsDev ds{du + o_nn, du + o_nt, du + o_t0, du + o_t1, dv, dv + S,
               st->incl_off ? du + o_io : nullptr, du + o_in, st->excl_off ? du + o_eo : nullptr, du + o_en};
-  StepOutDev dout{du + o_placed, h->d_st_sched.p, du + o_ooff, du + o_anode, du + o_antasks, dr + E,
+  StepOutDev dout{du + o_placed, h->d_steps_sched.p, du + o_ooff, du + o_anode, du + o_antasks, dr + E,
                   du + o_toff, du + o_tnode, dr + E + nrows};
   CU(cudaEventRecord(h->ev[kEvStepsBegin], sm));
   if (J) {
-    const uint32_t grid = std::min<uint32_t>((J + kStepWarps - 1) / kStepWarps, 16 * h->n_sm);
-    CRANE_LAUNCH(k_steps, grid, 32 * kStepWarps, 0, sm, dj, ds, dout, (uint32_t)h->dict_slot);
+    launch_steps(h, dj, ds, dout);
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(h->ev[kEvStepsEnd], sm));
   if (J) CU(cudaMemcpyAsync(out->placed, du + o_placed, J * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
-  if (S) CU(cudaMemcpyAsync(out->scheduled, h->d_st_sched.p, S, cudaMemcpyDeviceToHost, sm));
+  if (S) CU(cudaMemcpyAsync(out->scheduled, h->d_steps_sched.p, S, cudaMemcpyDeviceToHost, sm));
   if (nrows) {
     CU(cudaMemcpyAsync(out->alloc_node, du + o_anode, nrows * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
     CU(cudaMemcpyAsync(out->alloc_ntasks, du + o_antasks, nrows * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
@@ -2341,19 +2398,9 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jb, co
 int crane_sched_step_jobs_reset(crane_sched_t* h) {
   if (!h) return CRANE_EINVAL;
   TRY(require(h, kCluster, "step_jobs_reset"));
-  h->n_sj = h->n_sp = h->n_sa = 0;
-  h->h_sj_node_off.assign(1, 0);
-  h->h_sj_dead.clear();
-  h->h_sj_dirty.clear();
-  h->h_sj_queue.clear();
-  h->h_sj_dirty_rows.clear();
-  h->h_sp_job.clear();
-  h->h_sp_nn.clear();
-  h->h_sp_nt.clear();
-  h->h_sp_state.clear();
-  h->h_sp_incl_off.assign(1, 0);
-  h->h_sp_excl_off.assign(1, 0);
-  h->sp_results = false;
+  h->sj.reset();
+  h->sp.reset();
+  h->sr.valid = false;
   return CRANE_OK;
 }
 
@@ -2362,9 +2409,9 @@ int crane_sched_step_jobs_start(crane_sched_t* h, const uint32_t* rows, uint32_t
   TRY(require(h, kCluster, "step_jobs_start"));
   TRY(check_rows(h, "step_jobs_start", rows, n, h->rr.n, [&](uint32_t r) { return h->rr.h_dead[r] != 0; }));
   CU(cudaSetDevice(h->device));
-  h->sp_results = false;
+  h->sr.valid = false;
   cudaStream_t st = h->stream;
-  const uint32_t base = h->n_sj, eb = h->h_sj_node_off.back();
+  const uint32_t base = h->sj.n, eb = h->sj.h_node_off.back();
   std::vector<uint32_t> off(n + 1, eb);
   for (uint32_t k = 0; k < n; ++k) {
     const uint64_t e = (uint64_t)off[k] + (h->rr.h_rr_alloc_off[rows[k] + 1] - h->rr.h_rr_alloc_off[rows[k]]);
@@ -2372,21 +2419,21 @@ int crane_sched_step_jobs_start(crane_sched_t* h, const uint32_t* rows, uint32_t
     off[k + 1] = (uint32_t)e;
   }
   if (n) {
-    CU(h->d_sj_node.grow(off[n], eb, st));
-    CU(h->d_sj_avail.grow(off[n], eb, st));
-    H2D_AT(h->d_sj_node_off, off.data(), base, (size_t)n + 1);
+    CU(h->sj.d_node.grow(off[n], eb, st));
+    CU(h->sj.d_avail.grow(off[n], eb, st));
+    H2D_AT(h->sj.d_node_off, off.data(), base, (size_t)n + 1);
     H2D(h->d_sp_call, rows, n);
-    CU(h->d_sp_flag.ensure(1));
-    CU(cudaMemsetAsync(h->d_sp_flag.p, 0, sizeof(uint32_t), st));
+    CU(h->d_flag.ensure(1));
+    CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
     CRANE_LAUNCH(k_sj_seed, warp_grid(h, n), 256, 0, st, h->rr.d_rr_alloc_off.p, h->rr.d_rr_alloc_node.p, h->rr.d_rr_alloc_res.p,
-                 h->d_sp_call.p, n, h->d_sj_node_off.p + base, h->d_sj_node.p, h->d_sj_avail.p, h->d_sp_flag.p);
+                 h->d_sp_call.p, n, h->sj.d_node_off.p + base, h->sj.d_node.p, h->sj.d_avail.p, h->d_flag.p);
     uint32_t bad = 0;
-    CU(cudaMemcpyAsync(&bad, h->d_sp_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&bad, h->d_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     if (bad) return fail(h, CRANE_EINVAL, "step_jobs_start: a running row's allocation nodes are not ascending and distinct");
   }
-  sj_commit(h, off);
+  h->sj.commit(off);
   if (first) *first = base;
   return CRANE_OK;
 }
@@ -2395,28 +2442,20 @@ int crane_sched_step_jobs_append(crane_sched_t* h, const crane_step_jobs_t* jb, 
   if (!h || !jb) return CRANE_EINVAL;
   TRY(require(h, kCluster, "step_jobs_append"));
   if (jb->step_off) return fail(h, CRANE_EINVAL, "step_jobs_append: step_off must be NULL (steps come with steps_append)");
-  const uint32_t J = jb->n_jobs;
-  TRY(check_offsets(h, "step jobs: node_off", jb->node_off, J));
-  const uint32_t E = jb->node_off[J];
-  if (E && (!jb->node || !jb->avail)) return fail(h, CRANE_EINVAL, "step jobs: null node table");
-  for (uint32_t j = 0; j < J; ++j)
-    for (uint32_t k = jb->node_off[j]; k < jb->node_off[j + 1]; ++k) {
-      if (jb->node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "step jobs[%u]: node %u out of range", j, jb->node[k]);
-      if (k > jb->node_off[j] && jb->node[k] <= jb->node[k - 1])
-        return fail(h, CRANE_EINVAL, "step jobs[%u]: nodes must be ascending and distinct", j);
-    }
-  const uint32_t base = h->n_sj, eb = h->h_sj_node_off.back();
+  TRY(check_step_jobs(h, jb));
+  const uint32_t J = jb->n_jobs, E = jb->node_off[J];
+  const uint32_t base = h->sj.n, eb = h->sj.h_node_off.back();
   if ((uint64_t)eb + E > 0xfffffff0ull || (uint64_t)base + J > 0xfffffff0ull)
     return fail(h, CRANE_EINVAL, "step_jobs_append: too many rows");
   CU(cudaSetDevice(h->device));
-  h->sp_results = false;
+  h->sr.valid = false;
   std::vector<uint32_t> off(J + 1);
   for (uint32_t j = 0; j <= J; ++j) off[j] = eb + jb->node_off[j];
-  H2D_AT(h->d_sj_node_off, off.data(), base, (size_t)J + 1);
-  H2D_AT(h->d_sj_node, jb->node, eb, E);
-  H2D_AT(h->d_sj_avail, reinterpret_cast<const Row*>(jb->avail), eb, E);
+  H2D_AT(h->sj.d_node_off, off.data(), base, (size_t)J + 1);
+  H2D_AT(h->sj.d_node, jb->node, eb, E);
+  H2D_AT(h->sj.d_avail, reinterpret_cast<const Row*>(jb->avail), eb, E);
   CU(cudaStreamSynchronize(h->stream));  // (the staging vector is pageable)
-  sj_commit(h, off);
+  h->sj.commit(off);
   if (first) *first = base;
   return CRANE_OK;
 }
@@ -2424,11 +2463,11 @@ int crane_sched_step_jobs_append(crane_sched_t* h, const crane_step_jobs_t* jb, 
 int crane_sched_step_jobs_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n) {
   if (!h) return CRANE_EINVAL;
   TRY(require(h, kCluster, "step_jobs_erase"));
-  TRY(check_rows(h, "step_jobs_erase", rows, n, h->n_sj, [&](uint32_t r) { return h->h_sj_dead[r] != 0; }));
-  h->sp_results = false;
+  TRY(check_rows(h, "step_jobs_erase", rows, n, h->sj.n, [&](uint32_t r) { return h->sj.h_dead[r] != 0; }));
+  h->sr.valid = false;
   for (uint32_t k = 0; k < n; ++k) {  // its step rows go with it: every check looks at the job
-    h->h_sj_dead[rows[k]] = 1;
-    std::vector<uint32_t>().swap(h->h_sj_queue[rows[k]]);
+    h->sj.h_dead[rows[k]] = 1;
+    std::vector<uint32_t>().swap(h->sj.h_queue[rows[k]]);
   }
   return CRANE_OK;
 }
@@ -2441,44 +2480,44 @@ int crane_sched_steps_append(crane_sched_t* h, const crane_steps_t* st, const ui
   TRY(check_steps(h, st, &nrows, &trows));
   if (S && !job_row) return fail(h, CRANE_EINVAL, "steps_append: null job_row");
   for (uint32_t s = 0; s < S; ++s) {
-    if (job_row[s] >= h->n_sj) return fail(h, CRANE_EINVAL, "steps_append[%u]: job row %u out of range", s, job_row[s]);
-    if (h->h_sj_dead[job_row[s]]) return fail(h, CRANE_EINVAL, "steps_append[%u]: job row %u was erased", s, job_row[s]);
+    if (job_row[s] >= h->sj.n) return fail(h, CRANE_EINVAL, "steps_append[%u]: job row %u out of range", s, job_row[s]);
+    if (h->sj.h_dead[job_row[s]]) return fail(h, CRANE_EINVAL, "steps_append[%u]: job row %u was erased", s, job_row[s]);
   }
-  const uint32_t base = h->n_sp, ib = h->h_sp_incl_off.back(), xb = h->h_sp_excl_off.back();
+  const uint32_t base = h->sp.n, ib = h->sp.h_incl_off.back(), xb = h->sp.h_excl_off.back();
   const uint32_t ni = st->incl_off ? st->incl_off[S] : 0, nx = st->excl_off ? st->excl_off[S] : 0;
   if ((uint64_t)base + S > 0xfffffff0ull || (uint64_t)ib + ni > 0xfffffff0ull || (uint64_t)xb + nx > 0xfffffff0ull)
     return fail(h, CRANE_EINVAL, "steps_append: too many rows");
   CU(cudaSetDevice(h->device));
-  h->sp_results = false;
+  h->sr.valid = false;
   std::vector<uint32_t> io(S + 1), xo(S + 1);
   for (uint32_t s = 0; s <= S; ++s) {
     io[s] = ib + (st->incl_off ? st->incl_off[s] : 0);
     xo[s] = xb + (st->excl_off ? st->excl_off[s] : 0);
   }
-  H2D_AT(h->d_sp_job, job_row, base, S);
-  H2D_AT(h->d_sp_nn, st->node_num, base, S);
-  H2D_AT(h->d_sp_nt, st->ntasks, base, S);
-  H2D_AT(h->d_sp_t0, st->ntasks_per_node_min, base, S);
-  H2D_AT(h->d_sp_t1, st->ntasks_per_node_max, base, S);
-  H2D_AT(h->d_sp_req_node, reinterpret_cast<const View*>(st->req_node), base, S);
-  H2D_AT(h->d_sp_req_task, reinterpret_cast<const View*>(st->req_task), base, S);
-  H2D_AT(h->d_sp_incl_off, io.data(), base, (size_t)S + 1);
-  H2D_AT(h->d_sp_excl_off, xo.data(), base, (size_t)S + 1);
-  H2D_AT(h->d_sp_incl, st->incl_nodes, ib, ni);
-  H2D_AT(h->d_sp_excl, st->excl_nodes, xb, nx);
-  CU(h->d_sp_alloc_at.grow(std::max<size_t>((size_t)base + S, 1), base, h->stream));
+  H2D_AT(h->sp.d_job, job_row, base, S);
+  H2D_AT(h->sp.d_nn, st->node_num, base, S);
+  H2D_AT(h->sp.d_nt, st->ntasks, base, S);
+  H2D_AT(h->sp.d_t0, st->ntasks_per_node_min, base, S);
+  H2D_AT(h->sp.d_t1, st->ntasks_per_node_max, base, S);
+  H2D_AT(h->sp.d_req_node, reinterpret_cast<const View*>(st->req_node), base, S);
+  H2D_AT(h->sp.d_req_task, reinterpret_cast<const View*>(st->req_task), base, S);
+  H2D_AT(h->sp.d_incl_off, io.data(), base, (size_t)S + 1);
+  H2D_AT(h->sp.d_excl_off, xo.data(), base, (size_t)S + 1);
+  H2D_AT(h->sp.d_incl, st->incl_nodes, ib, ni);
+  H2D_AT(h->sp.d_excl, st->excl_nodes, xb, nx);
+  CU(h->sp.d_alloc_at.grow(std::max<size_t>((size_t)base + S, 1), base, h->stream));
   CU(cudaStreamSynchronize(h->stream));  // (the staging vectors are pageable)
   for (uint32_t s = 0; s < S; ++s) {
-    h->h_sp_job.push_back(job_row[s]);
-    h->h_sp_nn.push_back(st->node_num[s]);
-    h->h_sp_nt.push_back(st->ntasks[s]);
-    h->h_sp_state.push_back(kSpPending);
-    h->h_sp_incl_off.push_back(io[s + 1]);
-    h->h_sp_excl_off.push_back(xo[s + 1]);
-    h->h_sj_queue[job_row[s]].push_back(base + s);
-    sj_dirty(h, job_row[s]);
+    h->sp.h_job.push_back(job_row[s]);
+    h->sp.h_nn.push_back(st->node_num[s]);
+    h->sp.h_nt.push_back(st->ntasks[s]);
+    h->sp.h_state.push_back(kSpPending);
+    h->sp.h_incl_off.push_back(io[s + 1]);
+    h->sp.h_excl_off.push_back(xo[s + 1]);
+    h->sj.h_queue[job_row[s]].push_back(base + s);
+    h->sj.mark_dirty(job_row[s]);
   }
-  h->n_sp = base + S;
+  h->sp.n = base + S;
   if (first) *first = base;
   return CRANE_OK;
 }
@@ -2486,23 +2525,23 @@ int crane_sched_steps_append(crane_sched_t* h, const crane_steps_t* st, const ui
 int crane_sched_steps_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n) {
   if (!h) return CRANE_EINVAL;
   TRY(require(h, kCluster, "steps_erase"));
-  TRY(check_rows(h, "steps_erase", rows, n, h->n_sp, [&](uint32_t r) {
-    return h->h_sp_state[r] == kSpErased || h->h_sj_dead[h->h_sp_job[r]];
+  TRY(check_rows(h, "steps_erase", rows, n, h->sp.n, [&](uint32_t r) {
+    return h->sp.h_state[r] == kSpErased || h->sj.h_dead[h->sp.h_job[r]];
   }));
   CU(cudaSetDevice(h->device));
-  h->sp_results = false;
+  h->sr.valid = false;
   // scheduled rows give their node rows back, job by job, in row order
   std::vector<std::pair<uint32_t, uint32_t>> rel;  // (job, step row)
   for (uint32_t k = 0; k < n; ++k) {
-    const uint32_t s = rows[k], j = h->h_sp_job[s];
-    if (h->h_sp_state[s] == kSpScheduled) {
+    const uint32_t s = rows[k], j = h->sp.h_job[s];
+    if (h->sp.h_state[s] == kSpScheduled) {
       rel.emplace_back(j, s);
     } else {
-      auto& q = h->h_sj_queue[j];
+      auto& q = h->sj.h_queue[j];
       q.erase(std::find(q.begin(), q.end(), s));
     }
-    h->h_sp_state[s] = kSpErased;
-    sj_dirty(h, j);
+    h->sp.h_state[s] = kSpErased;
+    h->sj.mark_dirty(j);
   }
   if (rel.empty()) return CRANE_OK;
   std::sort(rel.begin(), rel.end());
@@ -2521,7 +2560,7 @@ int crane_sched_steps_erase(crane_sched_t* h, const uint32_t* rows, uint32_t n) 
   u.insert(u.end(), steps.begin(), steps.end());
   H2D(h->d_sp_call, u.data(), u.size());
   const uint32_t* du = h->d_sp_call.p;
-  CRANE_LAUNCH(k_sp_release, warp_grid(h, m), 256, 0, h->stream, step_pool(h), du, du + m, du + 2 * m + 1, m);
+  CRANE_LAUNCH(k_sp_release, warp_grid(h, m), 256, 0, h->stream, step_pool(h->sj, h->sp), du, du + m, du + 2 * m + 1, m);
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(h->stream));
   return CRANE_OK;
@@ -2534,35 +2573,32 @@ int crane_sched_steps_run(crane_sched_t* h, uint32_t* n_scheduled, uint32_t* n_n
   CU(cudaSetDevice(h->device));
   (void)cudaGetLastError();
   cudaStream_t sm = h->stream;
-  h->sp_results = false;
+  h->sr.clear();
+  h->sr.sa_base = h->sp.n_alloc;
   // the pass visits the dirty jobs with a live pending step, ascending, each with its queue
-  std::sort(h->h_sj_dirty_rows.begin(), h->h_sj_dirty_rows.end());
+  std::sort(h->sj.h_dirty_rows.begin(), h->sj.h_dirty_rows.end());
   std::vector<uint32_t> u;  // jl | sl
-  for (uint32_t j : h->h_sj_dirty_rows) {
-    h->h_sj_dirty[j] = 0;
-    if (!h->h_sj_dead[j] && !h->h_sj_queue[j].empty()) u.push_back(j);
+  for (uint32_t j : h->sj.h_dirty_rows) {
+    h->sj.h_dirty[j] = 0;
+    if (!h->sj.h_dead[j] && !h->sj.h_queue[j].empty()) u.push_back(j);
   }
-  h->h_sj_dirty_rows.clear();
+  h->sj.h_dirty_rows.clear();
   const uint32_t J = (uint32_t)u.size();
   uint64_t E = 0, Li = 0, Le = 0, N = 0, T = 0;
   for (uint32_t w = 0; w < J; ++w) {
     const uint32_t j = u[w];
-    E += h->h_sj_node_off[j + 1] - h->h_sj_node_off[j];
-    for (uint32_t s : h->h_sj_queue[j]) {
+    E += h->sj.h_node_off[j + 1] - h->sj.h_node_off[j];
+    for (uint32_t s : h->sj.h_queue[j]) {
       u.push_back(s);
-      Li += h->h_sp_incl_off[s + 1] - h->h_sp_incl_off[s];
-      Le += h->h_sp_excl_off[s + 1] - h->h_sp_excl_off[s];
-      N += h->h_sp_nn[s];
-      T += h->h_sp_nt[s];
+      Li += h->sp.h_incl_off[s + 1] - h->sp.h_incl_off[s];
+      Le += h->sp.h_excl_off[s + 1] - h->sp.h_excl_off[s];
+      N += h->sp.h_nn[s];
+      T += h->sp.h_nt[s];
     }
   }
   const uint32_t S = (uint32_t)(u.size() - J);
-  if (N > 0xfffffff0ull || T > 0xfffffff0ull || (uint64_t)h->n_sa + N > 0xfffffff0ull)
+  if (N > 0xfffffff0ull || T > 0xfffffff0ull || (uint64_t)h->sp.n_alloc + N > 0xfffffff0ull)
     return fail(h, CRANE_EINVAL, "steps_run: too many node / task rows");
-  h->h_sr_rows.clear();
-  h->h_sr_node_off.assign(1, 0);
-  h->h_sr_task_off.assign(1, 0);
-  h->sr_sa_base = h->n_sa;
   float ms = 0.f;
   if (J) {
     // dense u32 columns: jl | sl | node_off | node | step_off | nn | nt | t0 | t1 | incl_off | incl | excl_off | excl |
@@ -2574,12 +2610,12 @@ int crane_sched_steps_run(crane_sched_t* h, uint32_t* n_scheduled, uint32_t* n_n
     const size_t o_io = take(S + 1), o_in = take(Li), o_xo = take(S + 1), o_xn = take(Le);
     const size_t o_ooff = take(S + 1), o_toff = take(S + 1), o_placed = take(J);
     const size_t o_anode = take(N), o_antasks = take(N), o_tnode = take(T), o_pos = take(2 * (uint64_t)S);
-    CU(h->d_sq_u32.ensure(at));
-    CU(h->d_sq_rows.ensure(std::max<uint64_t>(E + N + T, 1)));
-    CU(h->d_sq_views.ensure(2 * (size_t)S));
-    CU(h->d_sq_sched.ensure(S));
-    uint32_t* du = h->d_sq_u32.p;
-    Row* dr = h->d_sq_rows.p;
+    CU(h->d_steps_u32.ensure(at));
+    CU(h->d_steps_rows.ensure(std::max<uint64_t>(E + N + T, 1)));
+    CU(h->d_steps_views.ensure(2 * (size_t)S));
+    CU(h->d_steps_sched.ensure(S));
+    uint32_t* du = h->d_steps_u32.p;
+    Row* dr = h->d_steps_rows.p;
     StepPassDev d{};
     d.n_jobs = J;
     d.n_steps = S;
@@ -2593,8 +2629,8 @@ int crane_sched_steps_run(crane_sched_t* h, uint32_t* n_scheduled, uint32_t* n_n
     d.ntasks = du + o_nt;
     d.ntpn_min = du + o_t0;
     d.ntpn_max = du + o_t1;
-    d.req_node = h->d_sq_views.p;
-    d.req_task = h->d_sq_views.p + S;
+    d.req_node = h->d_steps_views.p;
+    d.req_task = h->d_steps_views.p + S;
     d.incl_off = du + o_io;
     d.incl_nodes = du + o_in;
     d.excl_off = du + o_xo;
@@ -2602,7 +2638,7 @@ int crane_sched_steps_run(crane_sched_t* h, uint32_t* n_scheduled, uint32_t* n_n
     d.out_node_off = du + o_ooff;
     d.out_task_off = du + o_toff;
     d.placed = du + o_placed;
-    d.scheduled = h->d_sq_sched.p;
+    d.scheduled = h->d_steps_sched.p;
     d.alloc_node = du + o_anode;
     d.alloc_ntasks = du + o_antasks;
     d.task_node = du + o_tnode;
@@ -2611,17 +2647,16 @@ int crane_sched_steps_run(crane_sched_t* h, uint32_t* n_scheduled, uint32_t* n_n
     CU(cudaMemcpyAsync(du, u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, sm));
     CU(cudaEventRecord(h->ev[kEvSpBegin], sm));
     const uint32_t mx = std::max(J, S) + 1;
-    CRANE_LAUNCH(k_sp_pass_cols, std::min<uint32_t>((mx + 255) / 256, 8 * h->n_sm), 256, 0, sm, step_pool(h), d);
+    CRANE_LAUNCH(k_sp_pass_cols, std::min<uint32_t>((mx + 255) / 256, 8 * h->n_sm), 256, 0, sm, step_pool(h->sj, h->sp), d);
     ScanSegs sg{{d.node_off, d.incl_off, d.excl_off, d.out_node_off, d.out_task_off}, {J + 1, S + 1, S + 1, S + 1, S + 1}};
     CRANE_LAUNCH(k_sp_scan, 1, 1024, 0, sm, sg);
-    CRANE_LAUNCH(k_sp_pass_rows, warp_grid(h, (uint64_t)J + S), 256, 0, sm, step_pool(h), d);
+    CRANE_LAUNCH(k_sp_pass_rows, warp_grid(h, (uint64_t)J + S), 256, 0, sm, step_pool(h->sj, h->sp), d);
     StepJobsDev dj{J, d.node_off, d.node, d.avail, d.step_off};
     StepsDev ds{d.node_num, d.ntasks, d.ntpn_min, d.ntpn_max, d.req_node, d.req_task,
                 d.incl_off, d.incl_nodes, d.excl_off, d.excl_nodes};
     StepOutDev dout{d.placed, d.scheduled, d.out_node_off, d.alloc_node, d.alloc_ntasks, d.alloc_res,
                     d.out_task_off, d.task_node, d.task_res};
-    const uint32_t grid = std::min<uint32_t>((J + kStepWarps - 1) / kStepWarps, 16 * h->n_sm);
-    CRANE_LAUNCH(k_steps, grid, 32 * kStepWarps, 0, sm, dj, ds, dout, (uint32_t)h->dict_slot);
+    launch_steps(h, dj, ds, dout);
     CU(cudaEventRecord(h->ev[kEvSpMid], sm));
     std::vector<uint8_t> sched(S);
     CU(cudaMemcpyAsync(sched.data(), d.scheduled, S, cudaMemcpyDeviceToHost, sm));
@@ -2635,22 +2670,22 @@ int crane_sched_steps_run(crane_sched_t* h, uint32_t* n_scheduled, uint32_t* n_n
     std::vector<uint32_t> pos(2 * (size_t)S, 0);
     for (const auto& g : got) {
       const uint32_t s = g.first;
-      pos[2 * (size_t)g.second] = h->h_sr_node_off.back();
-      pos[2 * (size_t)g.second + 1] = h->h_sr_task_off.back();
-      h->h_sr_rows.push_back(s);
-      h->h_sr_node_off.push_back(h->h_sr_node_off.back() + h->h_sp_nn[s]);
-      h->h_sr_task_off.push_back(h->h_sr_task_off.back() + h->h_sp_nt[s]);
+      pos[2 * (size_t)g.second] = h->sr.h_node_off.back();
+      pos[2 * (size_t)g.second + 1] = h->sr.h_task_off.back();
+      h->sr.h_rows.push_back(s);
+      h->sr.h_node_off.push_back(h->sr.h_node_off.back() + h->sp.h_nn[s]);
+      h->sr.h_task_off.push_back(h->sr.h_task_off.back() + h->sp.h_nt[s]);
     }
-    const uint32_t Nr = h->h_sr_node_off.back(), Tr = h->h_sr_task_off.back();
+    const uint32_t Nr = h->sr.h_node_off.back(), Tr = h->sr.h_task_off.back();
     if (!got.empty()) {
-      CU(h->d_sa_node.grow((size_t)h->n_sa + Nr, h->n_sa, sm));
-      CU(h->d_sa_res.grow((size_t)h->n_sa + Nr, h->n_sa, sm));
-      CU(h->d_sr_u32.ensure((size_t)Nr + Tr));
-      CU(h->d_sr_rows.ensure(std::max<uint32_t>(Tr, 1)));
+      CU(h->sp.d_sa_node.grow((size_t)h->sp.n_alloc + Nr, h->sp.n_alloc, sm));
+      CU(h->sp.d_sa_res.grow((size_t)h->sp.n_alloc + Nr, h->sp.n_alloc, sm));
+      CU(h->sr.d_u32.ensure((size_t)Nr + Tr));
+      CU(h->sr.d_rows.ensure(std::max<uint32_t>(Tr, 1)));
       CU(cudaMemcpyAsync(du + o_pos, pos.data(), pos.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, sm));
       CU(cudaEventRecord(h->ev[kEvSpScatter], sm));
-      CRANE_LAUNCH(k_sp_scatter, warp_grid(h, (uint64_t)J + S), 256, 0, sm, step_pool(h), d, du + o_pos, h->n_sa,
-                   h->d_sr_u32.p, h->d_sr_u32.p + Nr, h->d_sr_rows.p);
+      CRANE_LAUNCH(k_sp_scatter, warp_grid(h, (uint64_t)J + S), 256, 0, sm, step_pool(h->sj, h->sp), d, du + o_pos,
+                   h->sp.n_alloc, h->sr.d_u32.p, h->sr.d_u32.p + Nr, h->sr.d_rows.p);
       CU(cudaEventRecord(h->ev[kEvSpEnd], sm));
       CU(cudaStreamSynchronize(sm));
       CU(cudaGetLastError());
@@ -2660,42 +2695,42 @@ int crane_sched_steps_run(crane_sched_t* h, uint32_t* n_scheduled, uint32_t* n_n
     // mirrors: the scheduled steps are the head of their job's queue
     uint32_t i = 0;
     for (uint32_t w = 0; w < J; ++w) {
-      auto& q = h->h_sj_queue[u[w]];
+      auto& q = h->sj.h_queue[u[w]];
       size_t k = 0;
-      for (const size_t len = q.size(); k < len && sched[i + k]; ++k) h->h_sp_state[q[k]] = kSpScheduled;
+      for (const size_t len = q.size(); k < len && sched[i + k]; ++k) h->sp.h_state[q[k]] = kSpScheduled;
       i += (uint32_t)q.size();
       q.erase(q.begin(), q.begin() + k);
     }
-    h->n_sa += Nr;
+    h->sp.n_alloc += Nr;
   }
-  if (n_scheduled) *n_scheduled = (uint32_t)h->h_sr_rows.size();
-  if (n_node_rows) *n_node_rows = h->h_sr_node_off.back();
-  if (n_task_rows) *n_task_rows = h->h_sr_task_off.back();
+  if (n_scheduled) *n_scheduled = (uint32_t)h->sr.h_rows.size();
+  if (n_node_rows) *n_node_rows = h->sr.h_node_off.back();
+  if (n_task_rows) *n_task_rows = h->sr.h_task_off.back();
   if (device_ms) *device_ms = ms;
-  h->sp_results = true;
+  h->sr.valid = true;
   return CRANE_OK;
 }
 
 int crane_sched_steps_fetch(crane_sched_t* h, crane_step_results_t* out) {
   if (!h || !out) return CRANE_EINVAL;
-  if (!h->sp_results) return fail(h, CRANE_EINVAL, "steps_fetch: steps_run first");
-  const size_t Ns = h->h_sr_rows.size(), N = h->h_sr_node_off.back(), T = h->h_sr_task_off.back();
+  if (!h->sr.valid) return fail(h, CRANE_EINVAL, "steps_fetch: steps_run first");
+  const size_t Ns = h->sr.h_rows.size(), N = h->sr.h_node_off.back(), T = h->sr.h_task_off.back();
   if (!out->node_off || !out->task_off || (Ns && !out->step_row) ||
       (N && (!out->alloc_node || !out->alloc_ntasks || !out->alloc_res)) || (T && (!out->task_node || !out->task_res)))
     return fail(h, CRANE_EINVAL, "step results: null column");
   CU(cudaSetDevice(h->device));
   cudaStream_t sm = h->stream;
-  if (Ns) memcpy(out->step_row, h->h_sr_rows.data(), Ns * sizeof(uint32_t));
-  memcpy(out->node_off, h->h_sr_node_off.data(), (Ns + 1) * sizeof(uint32_t));
-  memcpy(out->task_off, h->h_sr_task_off.data(), (Ns + 1) * sizeof(uint32_t));
+  if (Ns) memcpy(out->step_row, h->sr.h_rows.data(), Ns * sizeof(uint32_t));
+  memcpy(out->node_off, h->sr.h_node_off.data(), (Ns + 1) * sizeof(uint32_t));
+  memcpy(out->task_off, h->sr.h_task_off.data(), (Ns + 1) * sizeof(uint32_t));
   if (N) {
-    CU(cudaMemcpyAsync(out->alloc_node, h->d_sa_node.p + h->sr_sa_base, N * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
-    CU(cudaMemcpyAsync(out->alloc_res, h->d_sa_res.p + h->sr_sa_base, N * sizeof(Row), cudaMemcpyDeviceToHost, sm));
-    CU(cudaMemcpyAsync(out->alloc_ntasks, h->d_sr_u32.p, N * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->alloc_node, h->sp.d_sa_node.p + h->sr.sa_base, N * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->alloc_res, h->sp.d_sa_res.p + h->sr.sa_base, N * sizeof(Row), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->alloc_ntasks, h->sr.d_u32.p, N * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
   }
   if (T) {
-    CU(cudaMemcpyAsync(out->task_node, h->d_sr_u32.p + N, T * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
-    CU(cudaMemcpyAsync(out->task_res, h->d_sr_rows.p, T * sizeof(Row), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->task_node, h->sr.d_u32.p + N, T * sizeof(uint32_t), cudaMemcpyDeviceToHost, sm));
+    CU(cudaMemcpyAsync(out->task_res, h->sr.d_rows.p, T * sizeof(Row), cudaMemcpyDeviceToHost, sm));
   }
   CU(cudaStreamSynchronize(sm));
   return CRANE_OK;
@@ -2705,20 +2740,20 @@ int crane_sched_step_jobs_avail(crane_sched_t* h, const uint32_t* rows, uint32_t
                                 uint32_t* n_node_rows) {
   if (!h) return CRANE_EINVAL;
   TRY(require(h, kCluster, "step_jobs_avail"));
-  TRY(check_rows(h, "step_jobs_avail", rows, n, h->n_sj, [&](uint32_t r) { return h->h_sj_dead[r] != 0; }));
+  TRY(check_rows(h, "step_jobs_avail", rows, n, h->sj.n, [&](uint32_t r) { return h->sj.h_dead[r] != 0; }));
   std::vector<uint32_t> u(rows, rows + n);  // rows | dst_off
   u.push_back(0);
-  for (uint32_t k = 0; k < n; ++k) u.push_back(u.back() + h->h_sj_node_off[rows[k] + 1] - h->h_sj_node_off[rows[k]]);
+  for (uint32_t k = 0; k < n; ++k) u.push_back(u.back() + h->sj.h_node_off[rows[k] + 1] - h->sj.h_node_off[rows[k]]);
   const uint32_t E = u.back();
   if (n_node_rows) *n_node_rows = E;
   CU(cudaSetDevice(h->device));
-  h->sp_results = false;
+  h->sr.valid = false;
   if (!E || !dst) return CRANE_OK;
   H2D(h->d_sp_call, u.data(), u.size());
-  CU(h->d_sq_rows.ensure(E));
-  CRANE_LAUNCH(k_sj_avail_gather, warp_grid(h, n), 256, 0, h->stream, h->d_sj_node_off.p, h->d_sj_avail.p,
-               h->d_sp_call.p, h->d_sp_call.p + n, n, h->d_sq_rows.p);
-  CU(cudaMemcpyAsync(dst, h->d_sq_rows.p, (size_t)E * sizeof(Row), cudaMemcpyDeviceToHost, h->stream));
+  CU(h->d_steps_rows.ensure(E));
+  CRANE_LAUNCH(k_sj_avail_gather, warp_grid(h, n), 256, 0, h->stream, h->sj.d_node_off.p, h->sj.d_avail.p,
+               h->d_sp_call.p, h->d_sp_call.p + n, n, h->d_steps_rows.p);
+  CU(cudaMemcpyAsync(dst, h->d_steps_rows.p, (size_t)E * sizeof(Row), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
   CU(cudaGetLastError());
   return CRANE_OK;
