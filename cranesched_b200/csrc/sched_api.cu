@@ -447,6 +447,228 @@ struct StepResults {
   }
 };
 
+// Sizes buffers in turn, each to at least one element, and keeps the first error
+struct Sizes {
+  cudaError_t e = cudaSuccess;
+  template <class T>
+  void operator()(DBuf<T>& b, size_t n) {
+    if (e == cudaSuccess) e = b.ensure(std::max<size_t>(n, 1));
+  }
+};
+
+// The reservations of the cluster (crane_sched_set_reservations): each one's nodes,
+// ascending, with the resources it holds on them
+struct Reservations {
+  uint32_t n = 0;
+  std::vector<int64_t> start, end;
+  std::vector<uint32_t> node_off = {0}, node;
+  std::vector<Row> res;
+
+  void reset() {
+    n = 0;
+    start.clear();
+    end.clear();
+    node_off.assign(1, 0);
+    node.clear();
+    res.clear();
+  }
+};
+
+// The cluster as set_cluster and set_reservations store it, the slot layout of its node
+// states that build_layout derives from it, and the device copies of both with the
+// timelines. A new layout reuses the device buffers: the timelines alone hold
+// n_slots x tl_cap entries.
+struct ClusterLayout {
+  // the inputs
+  uint32_t n_nodes = 0, n_parts = 0;
+  GresDict dict{};
+  std::vector<Row> res_total;
+  std::vector<uint8_t> alive, drain;
+  std::vector<uint32_t> part_off, part_nodes;
+  Reservations resv;
+  uint32_t tl_cap = 0;  // timeline entries per node state: max_jobs_per_node + 1
+  // the slot layout
+  uint32_t n_slots = 0, max_part_slots = 0, words_per_row = 0, v2_ring = 0;
+  uint32_t n_vparts = 0;  // schedulers = groups of overlapping partitions + reservations
+  uint32_t n_comp = 0, max_comp_parts = 1;
+  std::vector<uint32_t> h_part_comp, h_part_cidx, h_sched_nparts, h_part_base, h_slot_node, h_node_slot;
+  // device copies
+  DBuf<uint32_t> d_part_base, d_slot_node, d_node_slot, d_slot_resv, d_rsv_off, d_rsv_id, d_sched_nparts, d_part_comp,
+      d_part_cidx, d_r_node_off, d_r_node;
+  DBuf<Row> d_slot_total, d_class_rows, d_rsv_res;
+  DBuf<uint8_t> d_slot_class, d_slot_memb;
+  DBuf<int64_t> d_resv_start, d_resv_end;
+  // the timelines
+  DBuf<uint32_t> d_tl_n;
+  DBuf<TlEntry> d_tl_ent;
+  DBuf<Row> d_avail0;
+  DBuf<double> d_cost0;
+  DBuf<uint8_t> d_skip;
+  DBuf<int64_t> d_first_resv;
+  // per scheduler: a run's queued jobs, k_commit2's profile counters
+  DBuf<uint32_t> d_part_count, d_part_job_off;
+  DBuf<unsigned long long> d_prof;
+
+  ClusterDev dev() const {
+    ClusterDev cl{};
+    cl.n_slots = n_slots;
+    cl.n_parts = n_parts;
+    cl.n_vparts = n_vparts;
+    cl.n_comp = n_comp;
+    cl.part_comp = d_part_comp.p;
+    cl.part_cidx = d_part_cidx.p;
+    cl.slot_memb = max_comp_parts > 1 ? d_slot_memb.p : nullptr;
+    cl.n_resv = resv.n;
+    cl.resv_start = d_resv_start.p;
+    cl.resv_end = d_resv_end.p;
+    cl.slot_resv = d_slot_resv.p;
+    cl.rsv_off = d_rsv_off.p;
+    cl.rsv_id = d_rsv_id.p;
+    cl.rsv_res = d_rsv_res.p;
+    cl.max_part_slots = max_part_slots;
+    cl.part_base = d_part_base.p;
+    cl.slot_node = d_slot_node.p;
+    cl.node_slot = d_node_slot.p;
+    cl.slot_total = d_slot_total.p;
+    cl.slot_class = d_slot_class.p;
+    cl.class_rows = d_class_rows.p;
+    return cl;
+  }
+
+  TimelineDev timelines() const {
+    TimelineDev tl{};
+    tl.cap = tl_cap;
+    tl.n = d_tl_n.p;
+    tl.ent = d_tl_ent.p;
+    tl.avail0 = d_avail0.p;
+    tl.cost0 = d_cost0.p;
+    tl.skip = d_skip.p;
+    tl.first_resv = d_first_resv.p;
+    return tl;
+  }
+
+  NodeStateMap node_states() const {
+    return NodeStateMap{n_nodes, n_slots, n_comp, resv.n, d_node_slot.p, d_part_base.p, d_r_node_off.p, d_r_node.p};
+  }
+};
+
+// The tick's view of the running table's live rows (RunningDev), built by the regroup:
+// their dense columns, their allocations grouped by node state, the jobs grouped by account
+struct RunView {
+  uint32_t n = 0, n_accounts = 0;  // live rows, accounts (pending rows' included)
+  RunCols rn;
+  DBuf<uint32_t> d_slot_off, d_acc_off, d_acc_job;
+  DBuf<int64_t> d_slot_end;
+  DBuf<Row> d_slot_res;
+  DBuf<uint64_t> d_acc_key;
+  DBuf<uint8_t> d_acc_present;
+
+  // R live rows with E allocation entries (tombstones' included), n_slots node states, A accounts
+  cudaError_t ensure(uint32_t R, uint32_t E, uint32_t n_slots, uint32_t A) {
+    Sizes s{ensure_cols(rn, R)};
+    s(d_acc_key, R);
+    s(d_acc_job, R);
+    s(d_slot_off, (size_t)n_slots + 1);
+    s(d_slot_end, E);
+    s(d_slot_res, E);
+    s(d_acc_off, (size_t)A + 1);
+    s(d_acc_present, A);
+    return s.e;
+  }
+
+  RunningDev dev() const {
+    RunningDev d{};
+    d.n = n;
+    d.start_time = rn.d_rr_start.p;
+    d.end_time = rn.d_rr_end.p;
+    d.node_num = rn.d_rr_node_num.p;
+    d.partition_priority = rn.d_rr_part_prio.p;
+    d.qos_priority = rn.d_rr_qos_prio.p;
+    d.account = rn.d_rr_account.p;
+    d.view_cpu_raw = rn.d_rr_cpu.p;
+    d.view_mem = rn.d_rr_mem.p;
+    d.slot_off = d_slot_off.p;
+    d.slot_end = d_slot_end.p;
+    d.slot_res = d_slot_res.p;
+    d.n_accounts = n_accounts;
+    d.acc_off = d_acc_off.p;
+    d.acc_job = d_acc_job.p;
+    d.acc_present = d_acc_present.p;
+    return d;
+  }
+};
+
+// The last run's placements of the pending rows (PlaceDev)
+struct RunOutputs {
+  DBuf<uint8_t> d_reason;
+  DBuf<double> d_prio;
+  DBuf<int64_t> d_start, d_end;
+  DBuf<uint32_t> d_nalloc, d_node, d_ntasks;  // per row | per allocation row
+  DBuf<Row> d_res;
+
+  cudaError_t ensure(size_t n_jobs, size_t n_alloc_rows) {
+    Sizes s;
+    s(d_reason, n_jobs);
+    s(d_prio, n_jobs);
+    s(d_start, n_jobs);
+    s(d_end, n_jobs);
+    s(d_nalloc, n_jobs);
+    s(d_node, n_alloc_rows);
+    s(d_ntasks, n_alloc_rows);
+    s(d_res, n_alloc_rows);
+    return s.e;
+  }
+
+  void release() {
+    d_reason.release(); d_prio.release(); d_start.release(); d_end.release();
+    d_nalloc.release(); d_node.release(); d_ntasks.release(); d_res.release();
+  }
+
+  PlaceDev dev() const {
+    return PlaceDev{d_reason.p, d_prio.p, d_start.p, d_end.p, d_nalloc.p, d_node.p, d_ntasks.p, d_res.p};
+  }
+};
+
+// The run's work buffers; the regroup, compaction and qos_filter sort in the priority
+// sort's keys and values. release() frees every buffer sized by the tables' rows, and
+// each is sized again before its next use: by ensure() in keep_running, by ensure_sort()
+// in the other calls that sort, by the run (d_vpart, d_g_code) or by radix_sort (d_hist).
+// d_bounds (one record) and d_acc_service (one entry per account) are not released.
+struct RunWork {
+  DBuf<Bounds> d_bounds;
+  DBuf<double> d_acc_service, d_prio;
+  DBuf<uint64_t> d_keys_a, d_keys_b;
+  DBuf<uint32_t> d_vals_a, d_vals_b, d_hist, d_vpart, d_bitmap;
+  DBuf<uint8_t> d_g_code;  // the run's exclusion code of every pending row (k_gate)
+  DBuf<JobQ> d_jobq;
+
+  cudaError_t ensure_sort(size_t n) {
+    Sizes s;
+    s(d_keys_a, n);
+    s(d_keys_b, n);
+    s(d_vals_a, n);
+    s(d_vals_b, n);
+    return s.e;
+  }
+
+  // N pending rows, sorts of n_sort keys, A accounts, nq queued jobs over bitmap rows of words_per_row
+  cudaError_t ensure(uint32_t N, size_t n_sort, uint32_t A, uint32_t nq, uint32_t words_per_row) {
+    Sizes s;
+    s(d_bounds, 1);
+    s(d_acc_service, A);
+    s(d_prio, N);
+    if (s.e == cudaSuccess) s.e = ensure_sort(n_sort);
+    s(d_jobq, nq);
+    s(d_bitmap, (size_t)std::max<uint32_t>(nq, 1) * words_per_row);
+    return s.e;
+  }
+
+  void release() {
+    d_keys_a.release(); d_keys_b.release(); d_vals_a.release(); d_vals_b.release(); d_hist.release();
+    d_prio.release(); d_vpart.release(); d_g_code.release(); d_jobq.release(); d_bitmap.release();
+  }
+};
+
 // How far a handle has got; each stage needs every earlier one. A call that replaces
 // the tables of a stage lowers the handle to the stage before it.
 enum Stage { kNone, kCluster, kUploaded, kRan };
@@ -478,80 +700,29 @@ struct crane_sched {
   size_t v2_budget = 0;       // dynamic shared memory k_commit2 may use
   uint32_t n_sm = 0;          // SMs of the device: grid caps of the grid-stride kernels
   bool h2d_timed = false;     // kEvH2dBegin, kEvH2dEnd were recorded (crane_sched_upload)
-  uint32_t v2_ring = 0;
   Stage stage = kNone;
+  int dict_slot = -1;  // this handle's entry of c_dicts[] on its device
 
-  // cluster (host copies)
-  uint32_t n_nodes = 0, n_parts = 0, n_slots = 0, max_part_slots = 0, words_per_row = 0;
-  uint32_t n_vparts = 0, n_resv = 0;  // schedulers = groups of overlapping partitions + reservations
-  uint32_t n_comp = 0, max_comp_parts = 1;
-  std::vector<uint32_t> h_part_comp, h_part_cidx, h_sched_nparts;
-  // host copies of the cluster and reservation tables (the slot layout is rebuilt when either changes)
-  std::vector<Row> c_res_total, r_res;
-  std::vector<uint8_t> c_alive, c_drain;
-  std::vector<uint32_t> c_part_off, c_part_nodes, r_node_off, r_node;
-  std::vector<int64_t> r_start, r_end;
-  std::vector<uint32_t> h_vslot_off, h_vslot_node;  // per reservation: its nodes (ascending) -> slots h_part_base[n_parts + r] + k
-  uint32_t n_gres_entries = 0;
-  std::vector<uint32_t> h_part_base, h_slot_node, h_node_slot;
-  GresDict dict{};
-  uint32_t tl_cap = 0;
-
-  // cluster (device)
-  DBuf<uint32_t> d_part_base, d_slot_node, d_node_slot;
-  DBuf<Row> d_slot_total;
-  // timelines
-  DBuf<uint32_t> d_tl_n;
-  DBuf<TlEntry> d_tl_ent;
-  DBuf<Row> d_avail0, d_class_rows;
-  DBuf<uint8_t> d_slot_class;
-  DBuf<double> d_cost0;
-  DBuf<uint8_t> d_skip;
-  DBuf<int64_t> d_first_resv, d_resv_start, d_resv_end;
-  DBuf<uint32_t> d_q_off;
-  DBuf<uint32_t> d_slot_resv, d_rsv_off, d_rsv_id, d_vpart, d_sched_nparts, d_part_comp, d_part_cidx, d_sched_owner;
-  DBuf<uint8_t> d_slot_memb;
-  DBuf<Row> d_rsv_res;
-
+  ClusterLayout layout;
   // the resident tables
   PendingTable pd;
   GateRows gate;
   DepEntries ent;
   RunningTable rr;
-  uint32_t n_running = 0, n_accounts = 0;  // the tick's live running rows, accounts
-  DBuf<uint32_t> d_erase_rows, d_r_node_off, d_r_node, d_flag, d_start_rows;
-  // the tick's view of the live rows (RunningDev), built by the regroup
-  RunCols rn;
-  DBuf<int64_t> d_rn_slot_end;
-  DBuf<uint32_t> d_rn_slot_off, d_rn_acc_off, d_rn_acc_job;
-  DBuf<uint64_t> d_rn_acc_key;
-  DBuf<Row> d_rn_slot_res;
-  DBuf<uint8_t> d_acc_present;
-  DBuf<uint8_t> d_g_code;  // the run's exclusion code of every pending row (k_gate)
+  // the run: its view of the running table, work buffers and placements
+  RunView view;
+  RunWork work;
+  RunOutputs outputs;
+  DBuf<uint32_t> d_erase_rows, d_start_rows, d_flag;  // per call: erased rows, started rows, a device flag
   DBuf<uint32_t> d_ev_rows, d_ev_u32;  // per call: sorted rows + their positions | exit codes, offsets
   DBuf<int64_t> d_ev_i64;              // per call: end / event times, begin times
   DBuf<uint8_t> d_ev_u8;               // per call: held, is_or
-  // work buffers
-  DBuf<Bounds> d_bounds;
-  DBuf<double> d_acc_service, d_prio;
-  DBuf<uint64_t> d_keys_a, d_keys_b;
-  DBuf<uint32_t> d_vals_a, d_vals_b, d_hist, d_part_count, d_part_job_off, d_bitmap;
-  DBuf<JobQ> d_jobq;
-  DBuf<unsigned long long> d_prof;
-  uint32_t* d_queue = nullptr;  // points into vals_a / vals_b after the sorts
-  // outputs (device)
-  DBuf<uint8_t> d_reason;
-  DBuf<double> d_out_prio;
-  DBuf<int64_t> d_out_start, d_out_end;
-  DBuf<uint32_t> d_out_nalloc, d_out_node, d_out_ntasks;
-  DBuf<Row> d_out_res;
-  int dict_slot = -1;  // this handle's entry of c_dicts[] on its device
   // one queue over several GPUs
   uint32_t shard_rank = 0, shard_n = 1;
   std::vector<uint32_t> h_part_owner, h_part_list;
-  DBuf<uint32_t> d_part_owner, d_part_list;
+  DBuf<uint32_t> d_part_owner, d_part_list, d_sched_owner;
   // QoS post-filter (R12)
-  DBuf<uint32_t> d_q_u32, d_q_chain_off, d_q_chain;
+  DBuf<uint32_t> d_q_off, d_q_u32, d_q_chain_off, d_q_chain;
   DBuf<int64_t> d_q_i64;
   DBuf<uint8_t> d_q_valid;
   DBuf<crane_tres_limit_t> d_q_tres;
@@ -630,7 +801,7 @@ int check_node_list(crane_sched* h, const char* what, const uint32_t* off, const
   TRY(check_offsets(h, what, off, n));
   if (off[n] && !nodes) return fail(h, CRANE_EINVAL, "%s: node list CSR without node array", what);
   for (uint32_t k = 0; k < off[n]; ++k)
-    if (nodes[k] >= h->n_nodes && nodes[k] != 0xFFFFFFFFu) return fail(h, CRANE_EINVAL, "%s: listed node out of range", what);
+    if (nodes[k] >= h->layout.n_nodes && nodes[k] != 0xFFFFFFFFu) return fail(h, CRANE_EINVAL, "%s: listed node out of range", what);
   return CRANE_OK;
 }
 
@@ -686,16 +857,16 @@ int h2d(crane_sched* h, DBuf<T>& dst, const T* src, size_t n) {
 // stable LSD radix sort over bits [0, nbits) of d_keys_a with payload
 // d_vals_a; result pointers returned in keys/vals.
 int radix_sort(crane_sched* h, uint32_t n, int nbits, uint64_t** keys, uint32_t** vals) {
-  uint64_t* ka = h->d_keys_a.p;
-  uint64_t* kb = h->d_keys_b.p;
-  uint32_t* va = h->d_vals_a.p;
-  uint32_t* vb = h->d_vals_b.p;
+  uint64_t* ka = h->work.d_keys_a.p;
+  uint64_t* kb = h->work.d_keys_b.p;
+  uint32_t* va = h->work.d_vals_a.p;
+  uint32_t* vb = h->work.d_vals_b.p;
   uint32_t nblocks = (n + kSortTile - 1) / kSortTile;
-  CU(h->d_hist.ensure((size_t)256 * nblocks));
+  CU(h->work.d_hist.ensure((size_t)256 * nblocks));
   for (int shift = 0; shift < nbits; shift += 8) {
-    CRANE_LAUNCH(k_sort_hist, nblocks, 256, 0, h->stream, ka, n, shift, h->d_hist.p, nblocks);
-    CRANE_LAUNCH(k_sort_scan, 1, 1024, 0, h->stream, h->d_hist.p, 256u * nblocks);
-    CRANE_LAUNCH(k_sort_scatter, nblocks, 32, 0, h->stream, ka, va, kb, vb, n, shift, h->d_hist.p, nblocks);
+    CRANE_LAUNCH(k_sort_hist, nblocks, 256, 0, h->stream, ka, n, shift, h->work.d_hist.p, nblocks);
+    CRANE_LAUNCH(k_sort_scan, 1, 1024, 0, h->stream, h->work.d_hist.p, 256u * nblocks);
+    CRANE_LAUNCH(k_sort_scatter, nblocks, 32, 0, h->stream, ka, va, kb, vb, n, shift, h->work.d_hist.p, nblocks);
     h->timing.kernel_launches += 3;
     std::swap(ka, kb);
     std::swap(va, vb);
@@ -715,124 +886,125 @@ int gather(crane_sched* h, const ColSet& cs, const uint32_t* live, uint32_t n) {
 // Slot layout of the node states: the usable nodes of every partition (contiguous per
 // partition), then the nodes of every reservation; device copies of the cluster tables.
 int build_layout(crane_sched* h) {
-  h->h_node_slot.assign(h->n_nodes, 0xffffffffu);
-  h->h_slot_node.clear();
+  ClusterLayout& L = h->layout;
+  L.h_node_slot.assign(L.n_nodes, 0xffffffffu);
+  L.h_slot_node.clear();
   std::vector<Row> slot_total;
   uint32_t max_mp = 0;
   // Partitions that share a node share its NodeState (JobScheduler.cpp:5622): their job
   // loops are coupled through its timeline, so one scheduler (one CTA) takes every
   // connected component of overlapping partitions; each partition keeps its own order.
-  std::vector<uint32_t> uf(h->n_parts);
-  for (uint32_t p = 0; p < h->n_parts; ++p) uf[p] = p;
+  std::vector<uint32_t> uf(L.n_parts);
+  for (uint32_t p = 0; p < L.n_parts; ++p) uf[p] = p;
   auto find = [&](uint32_t x) { while (uf[x] != x) { uf[x] = uf[uf[x]]; x = uf[x]; } return x; };
   {
-    std::vector<uint32_t> first(h->n_nodes, 0xffffffffu);
-    for (uint32_t p = 0; p < h->n_parts; ++p) {
+    std::vector<uint32_t> first(L.n_nodes, 0xffffffffu);
+    for (uint32_t p = 0; p < L.n_parts; ++p) {
       uint32_t prev = 0;
-      for (uint32_t k = h->c_part_off[p]; k < h->c_part_off[p + 1]; ++k) {
-        const uint32_t n = h->c_part_nodes[k];
-        if (n >= h->n_nodes) return fail(h, CRANE_EINVAL, "cluster: node index %u out of range", n);
-        if (k > h->c_part_off[p] && n <= prev) return fail(h, CRANE_EINVAL, "cluster: partition %u node list must be ascending", p);
+      for (uint32_t k = L.part_off[p]; k < L.part_off[p + 1]; ++k) {
+        const uint32_t n = L.part_nodes[k];
+        if (n >= L.n_nodes) return fail(h, CRANE_EINVAL, "cluster: node index %u out of range", n);
+        if (k > L.part_off[p] && n <= prev) return fail(h, CRANE_EINVAL, "cluster: partition %u node list must be ascending", p);
         prev = n;
         if (first[n] == 0xffffffffu) first[n] = p;
         else { const uint32_t a = find(first[n]), c = find(p); if (a != c) uf[std::max(a, c)] = std::min(a, c); }
       }
     }
   }
-  h->h_part_comp.assign(h->n_parts, 0);
-  h->h_part_cidx.assign(h->n_parts, 0);
-  h->h_sched_nparts.clear();
+  L.h_part_comp.assign(L.n_parts, 0);
+  L.h_part_cidx.assign(L.n_parts, 0);
+  L.h_sched_nparts.clear();
   std::vector<std::vector<uint32_t>> comp_parts;
   {
-    std::vector<uint32_t> id(h->n_parts, 0xffffffffu);
-    for (uint32_t p = 0; p < h->n_parts; ++p) {
+    std::vector<uint32_t> id(L.n_parts, 0xffffffffu);
+    for (uint32_t p = 0; p < L.n_parts; ++p) {
       const uint32_t r = find(p);
       if (id[r] == 0xffffffffu) { id[r] = (uint32_t)comp_parts.size(); comp_parts.emplace_back(); }
-      h->h_part_comp[p] = id[r];
-      h->h_part_cidx[p] = (uint32_t)comp_parts[id[r]].size();
+      L.h_part_comp[p] = id[r];
+      L.h_part_cidx[p] = (uint32_t)comp_parts[id[r]].size();
       comp_parts[id[r]].push_back(p);
     }
   }
-  h->n_comp = (uint32_t)comp_parts.size();
-  h->h_part_base.assign(h->n_comp + 1, 0);
-  h->h_part_base.reserve(h->n_comp + h->n_resv + 1);
+  L.n_comp = (uint32_t)comp_parts.size();
+  L.h_part_base.assign(L.n_comp + 1, 0);
+  L.h_part_base.reserve(L.n_comp + L.resv.n + 1);
   std::vector<uint8_t> slot_memb;
   uint32_t max_cp = 1;
-  for (uint32_t c = 0; c < h->n_comp; ++c) {
-    h->h_part_base[c] = (uint32_t)h->h_slot_node.size();
+  for (uint32_t c = 0; c < L.n_comp; ++c) {
+    L.h_part_base[c] = (uint32_t)L.h_slot_node.size();
     if (comp_parts[c].size() > (size_t)kMaxCompParts)
       return fail(h, CRANE_ENOSYS, "cluster: %zu partitions overlap in one connected group (at most %d)", comp_parts[c].size(), kMaxCompParts);
     max_cp = std::max<uint32_t>(max_cp, (uint32_t)comp_parts[c].size());
-    h->h_sched_nparts.push_back((uint32_t)comp_parts[c].size());
+    L.h_sched_nparts.push_back((uint32_t)comp_parts[c].size());
     std::vector<std::pair<uint32_t, uint8_t>> nodes;  // (node, membership bits), ascending node index
     for (uint32_t i = 0; i < comp_parts[c].size(); ++i) {
       const uint32_t p = comp_parts[c][i];
-      for (uint32_t k = h->c_part_off[p]; k < h->c_part_off[p + 1]; ++k) nodes.push_back({h->c_part_nodes[k], (uint8_t)(1u << i)});
+      for (uint32_t k = L.part_off[p]; k < L.part_off[p + 1]; ++k) nodes.push_back({L.part_nodes[k], (uint8_t)(1u << i)});
     }
     std::sort(nodes.begin(), nodes.end());
     for (size_t i = 0; i < nodes.size();) {
       const uint32_t n = nodes[i].first;
       uint8_t bits = 0;
       for (; i < nodes.size() && nodes[i].first == n; ++i) bits |= nodes[i].second;
-      if (!h->c_alive[n] || h->c_drain[n]) continue;  // JobScheduler.cpp:5629
-      const Row& t = h->c_res_total[n];
+      if (!L.alive[n] || L.drain[n]) continue;  // JobScheduler.cpp:5629
+      const Row& t = L.res_total[n];
       if (t.cpu_raw < 0 || t.cpu_raw > (int64_t)1 << 40) return fail(h, CRANE_EINVAL, "cluster: node %u cpu out of range", n);
-      for (uint32_t e = h->n_gres_entries; e < CRANE_GRES_ENTRIES; ++e)
+      for (uint32_t e = L.dict.n_entries; e < CRANE_GRES_ENTRIES; ++e)
         if (field16(t.g, e)) return fail(h, CRANE_EINVAL, "cluster: node %u has slots for an undeclared gres entry", n);
-      h->h_node_slot[n] = (uint32_t)h->h_slot_node.size();
-      h->h_slot_node.push_back(n);
+      L.h_node_slot[n] = (uint32_t)L.h_slot_node.size();
+      L.h_slot_node.push_back(n);
       slot_total.push_back(t);
       slot_memb.push_back(bits);
     }
-    max_mp = std::max(max_mp, (uint32_t)h->h_slot_node.size() - h->h_part_base[c]);
+    max_mp = std::max(max_mp, (uint32_t)L.h_slot_node.size() - L.h_part_base[c]);
   }
-  h->h_part_base[h->n_comp] = (uint32_t)h->h_slot_node.size();
-  h->max_comp_parts = max_cp;
-  const uint32_t n_phys = (uint32_t)h->h_slot_node.size();
+  L.h_part_base[L.n_comp] = (uint32_t)L.h_slot_node.size();
+  L.max_comp_parts = max_cp;
+  const uint32_t n_phys = (uint32_t)L.h_slot_node.size();
   // one more scheduler per reservation: node states holding exactly the reserved
   // resources (JobScheduler.cpp:5689-5703), whatever the node's own state
-  h->n_vparts = h->n_comp + h->n_resv;
+  L.n_vparts = L.n_comp + L.resv.n;
   std::vector<uint32_t> slot_resv(n_phys, 0xffffffffu);
-  for (uint32_t r = 0; r < h->n_resv; ++r) {
-    for (uint32_t k = h->r_node_off[r]; k < h->r_node_off[r + 1]; ++k) {
-      h->h_slot_node.push_back(h->r_node[k]);
-      slot_total.push_back(h->r_res[k]);
+  for (uint32_t r = 0; r < L.resv.n; ++r) {
+    for (uint32_t k = L.resv.node_off[r]; k < L.resv.node_off[r + 1]; ++k) {
+      L.h_slot_node.push_back(L.resv.node[k]);
+      slot_total.push_back(L.resv.res[k]);
       slot_resv.push_back(r);
       slot_memb.push_back(1);
     }
-    h->h_sched_nparts.push_back(1);
-    h->h_part_base.push_back((uint32_t)h->h_slot_node.size());
-    max_mp = std::max(max_mp, h->r_node_off[r + 1] - h->r_node_off[r]);
+    L.h_sched_nparts.push_back(1);
+    L.h_part_base.push_back((uint32_t)L.h_slot_node.size());
+    max_mp = std::max(max_mp, L.resv.node_off[r + 1] - L.resv.node_off[r]);
   }
   // reservations holding resources of a partition's node, ascending reservation id
-  std::vector<uint32_t> rsv_off((size_t)h->h_slot_node.size() + 1, 0), rsv_id;
+  std::vector<uint32_t> rsv_off((size_t)L.h_slot_node.size() + 1, 0), rsv_id;
   std::vector<Row> rsv_res;
   {
     std::vector<std::vector<std::pair<uint32_t, uint32_t>>> per(n_phys);
-    for (uint32_t r = 0; r < h->n_resv; ++r)
-      for (uint32_t k = h->r_node_off[r]; k < h->r_node_off[r + 1]; ++k) {
-        const uint32_t g = h->h_node_slot[h->r_node[k]];
+    for (uint32_t r = 0; r < L.resv.n; ++r)
+      for (uint32_t k = L.resv.node_off[r]; k < L.resv.node_off[r + 1]; ++k) {
+        const uint32_t g = L.h_node_slot[L.resv.node[k]];
         if (g != 0xffffffffu) per[g].push_back({r, k});  // (nodes outside node_state_map are skipped, :5680)
       }
     for (uint32_t g = 0; g < n_phys; ++g) {
-      for (auto& e : per[g]) { rsv_id.push_back(e.first); rsv_res.push_back(h->r_res[e.second]); }
+      for (auto& e : per[g]) { rsv_id.push_back(e.first); rsv_res.push_back(L.resv.res[e.second]); }
       rsv_off[g + 1] = (uint32_t)rsv_id.size();
     }
-    for (size_t g = n_phys; g < h->h_slot_node.size(); ++g) rsv_off[g + 1] = (uint32_t)rsv_id.size();
+    for (size_t g = n_phys; g < L.h_slot_node.size(); ++g) rsv_off[g + 1] = (uint32_t)rsv_id.size();
   }
-  h->n_slots = (uint32_t)h->h_slot_node.size();
-  h->max_part_slots = max_mp;
-  h->words_per_row = std::max<uint32_t>(4, ((max_mp + 31) / 32 + 3) / 4 * 4);  // 16-byte rows for the bulk copies
-  h->v2_ring = commit2_ring_slots(max_mp, h->words_per_row, h->n_gres_entries > 0, h->v2_budget, h->max_comp_parts);
-  if (max_mp > 65000 || h->v2_ring == 0)
+  L.n_slots = (uint32_t)L.h_slot_node.size();
+  L.max_part_slots = max_mp;
+  L.words_per_row = std::max<uint32_t>(4, ((max_mp + 31) / 32 + 3) / 4 * 4);  // 16-byte rows for the bulk copies
+  L.v2_ring = commit2_ring_slots(max_mp, L.words_per_row, L.dict.n_entries > 0, h->v2_budget, L.max_comp_parts);
+  if (max_mp > 65000 || L.v2_ring == 0)
     return fail(h, CRANE_ENOSYS, "cluster: partition with %u usable nodes exceeds the per-SM state budget", max_mp);
   // res_total classes per partition (distinct rows), cached in shared memory by the commit kernel
   std::vector<uint8_t> slot_class(std::max<size_t>(slot_total.size(), 1), 0xff);
-  std::vector<Row> class_rows((size_t)std::max<uint32_t>(h->n_vparts, 1) * kMaxClasses);
+  std::vector<Row> class_rows((size_t)std::max<uint32_t>(L.n_vparts, 1) * kMaxClasses);
   memset(class_rows.data(), 0, class_rows.size() * sizeof(Row));
-  for (uint32_t p = 0; p < h->n_vparts; ++p) {
+  for (uint32_t p = 0; p < L.n_vparts; ++p) {
     uint32_t ncls = 0;
-    for (uint32_t g = h->h_part_base[p]; g < h->h_part_base[p + 1]; ++g) {
+    for (uint32_t g = L.h_part_base[p]; g < L.h_part_base[p + 1]; ++g) {
       uint32_t k = 0;
       for (; k < ncls; ++k)
         if (memcmp(&class_rows[(size_t)p * kMaxClasses + k], &slot_total[g], sizeof(Row)) == 0) break;
@@ -844,34 +1016,35 @@ int build_layout(crane_sched* h) {
     }
   }
 
-  H2D(h->d_part_base, h->h_part_base.data(), h->h_part_base.size());
-  H2D(h->d_slot_node, h->h_slot_node.data(), h->h_slot_node.size());
-  H2D(h->d_node_slot, h->h_node_slot.data(), h->h_node_slot.size());
-  H2D(h->d_slot_total, slot_total.data(), slot_total.size());
-  H2D(h->d_slot_class, slot_class.data(), slot_class.size());
-  H2D(h->d_class_rows, class_rows.data(), class_rows.size());
-  H2D(h->d_slot_resv, slot_resv.data(), slot_resv.size());
-  H2D(h->d_slot_memb, slot_memb.data(), slot_memb.size());
-  H2D(h->d_sched_nparts, h->h_sched_nparts.data(), h->h_sched_nparts.size());
-  H2D(h->d_part_comp, h->h_part_comp.data(), h->h_part_comp.size());
-  H2D(h->d_part_cidx, h->h_part_cidx.data(), h->h_part_cidx.size());
-  H2D(h->d_rsv_off, rsv_off.data(), rsv_off.size());
-  H2D(h->d_rsv_id, rsv_id.data(), rsv_id.size());
-  H2D(h->d_rsv_res, rsv_res.data(), rsv_res.size());
-  H2D(h->d_resv_start, h->r_start.data(), h->r_start.size());
-  H2D(h->d_resv_end, h->r_end.data(), h->r_end.size());
-  H2D(h->d_r_node_off, h->r_node_off.data(), h->r_node_off.size());
-  H2D(h->d_r_node, h->r_node.data(), h->r_node.size());
-  CU(cudaMemcpyToSymbolAsync(c_dicts, &h->dict, sizeof(GresDict), (size_t)h->dict_slot * sizeof(GresDict), cudaMemcpyHostToDevice, h->stream));
-  size_t ns = std::max<uint32_t>(h->n_slots, 1);
-  CU(h->d_tl_n.ensure(ns));
-  CU(h->d_tl_ent.ensure(ns * h->tl_cap));
-  CU(h->d_avail0.ensure(ns));
-  CU(h->d_cost0.ensure(ns));
-  CU(h->d_skip.ensure(ns));
-  CU(h->d_first_resv.ensure(ns));
-  CU(h->d_part_count.ensure(h->n_vparts + 2));
-  CU(h->d_part_job_off.ensure(h->n_vparts + 2));
+  H2D(L.d_part_base, L.h_part_base.data(), L.h_part_base.size());
+  H2D(L.d_slot_node, L.h_slot_node.data(), L.h_slot_node.size());
+  H2D(L.d_node_slot, L.h_node_slot.data(), L.h_node_slot.size());
+  H2D(L.d_slot_total, slot_total.data(), slot_total.size());
+  H2D(L.d_slot_class, slot_class.data(), slot_class.size());
+  H2D(L.d_class_rows, class_rows.data(), class_rows.size());
+  H2D(L.d_slot_resv, slot_resv.data(), slot_resv.size());
+  H2D(L.d_slot_memb, slot_memb.data(), slot_memb.size());
+  H2D(L.d_sched_nparts, L.h_sched_nparts.data(), L.h_sched_nparts.size());
+  H2D(L.d_part_comp, L.h_part_comp.data(), L.h_part_comp.size());
+  H2D(L.d_part_cidx, L.h_part_cidx.data(), L.h_part_cidx.size());
+  H2D(L.d_rsv_off, rsv_off.data(), rsv_off.size());
+  H2D(L.d_rsv_id, rsv_id.data(), rsv_id.size());
+  H2D(L.d_rsv_res, rsv_res.data(), rsv_res.size());
+  H2D(L.d_resv_start, L.resv.start.data(), L.resv.start.size());
+  H2D(L.d_resv_end, L.resv.end.data(), L.resv.end.size());
+  H2D(L.d_r_node_off, L.resv.node_off.data(), L.resv.node_off.size());
+  H2D(L.d_r_node, L.resv.node.data(), L.resv.node.size());
+  CU(cudaMemcpyToSymbolAsync(c_dicts, &L.dict, sizeof(GresDict), (size_t)h->dict_slot * sizeof(GresDict), cudaMemcpyHostToDevice, h->stream));
+  size_t ns = std::max<uint32_t>(L.n_slots, 1);
+  CU(L.d_tl_n.ensure(ns));
+  CU(L.d_tl_ent.ensure(ns * L.tl_cap));
+  CU(L.d_avail0.ensure(ns));
+  CU(L.d_cost0.ensure(ns));
+  CU(L.d_skip.ensure(ns));
+  CU(L.d_first_resv.ensure(ns));
+  CU(L.d_part_count.ensure(L.n_vparts + 2));
+  CU(L.d_part_job_off.ensure(L.n_vparts + 2));
+  CU(L.d_prof.ensure((size_t)L.n_vparts * 16));
   CU(cudaStreamSynchronize(h->stream));
   h->stage = kCluster;
   h->rr.dirty = true;  // the running view is grouped by node state
@@ -999,7 +1172,7 @@ int running_check(crane_sched* h, const crane_running_t* rn, bool replace) {
   for (uint32_t j = 0; j < R; ++j) {
     if (rn->account[j] > (1u << 24)) return fail(h, CRANE_EINVAL, "account ids must be dense (< 2^24)");
     for (uint32_t k = rn->alloc_off[j]; k < rn->alloc_off[j + 1]; ++k)
-      if (rn->alloc_node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "running[%u]: node out of range", j);
+      if (rn->alloc_node[k] >= h->layout.n_nodes) return fail(h, CRANE_EINVAL, "running[%u]: node out of range", j);
   }
   return CRANE_OK;
 }
@@ -1043,12 +1216,8 @@ int regroup(crane_sched* h, uint32_t R, uint32_t max_rn_account) {
   cudaStream_t st = h->stream;
   const uint32_t Rt = h->rr.n, E = h->rr.h_rr_alloc_off.back();
   const RunTableDev rt = h->rr.dev();
-  CU(ensure_cols(h->rn, R));
-  CU(h->d_rn_acc_key.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_acc_job.ensure(std::max<uint32_t>(R, 1)));
-  CU(h->d_rn_slot_off.ensure((size_t)h->n_slots + 1));
-  CU(h->d_rn_slot_end.ensure(std::max<uint32_t>(E, 1)));
-  CU(h->d_rn_slot_res.ensure(std::max<uint32_t>(E, 1)));
+  const ClusterLayout& L = h->layout;
+  RunView& v = h->view;
   CU(h->d_flag.ensure(1));
   CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
   uint64_t* keys;
@@ -1057,39 +1226,38 @@ int regroup(crane_sched* h, uint32_t R, uint32_t max_rn_account) {
   if (R) {
     vals = nullptr;
     if (h->rr.n_dead) {
-      CRANE_LAUNCH(k_rt_live_keys, (Rt + 255) / 256, 256, 0, st, rt.dead, Rt, h->d_keys_a.p, h->d_vals_a.p);
+      CRANE_LAUNCH(k_rt_live_keys, (Rt + 255) / 256, 256, 0, st, rt.dead, Rt, h->work.d_keys_a.p, h->work.d_vals_a.p);
       TRY(radix_sort(h, Rt, 8, &keys, &vals));
     }
     ColSet cs{};
-    h->rr.RunCols::each(h->rn, gather_to(cs, R));
+    h->rr.RunCols::each(v.rn, gather_to(cs, R));
     TRY(gather(h, cs, vals, R));
   }
   // allocations by node state: stable sort of the entries (row order) by slot
   if (E) {
-    NodeStateMap m{h->n_nodes, h->n_slots, h->n_comp, h->n_resv, h->d_node_slot.p, h->d_part_base.p, h->d_r_node_off.p, h->d_r_node.p};
     const uint32_t nb = std::min<uint32_t>((Rt + 7) / 8, 8 * h->n_sm);
-    CRANE_LAUNCH(k_rt_entry_keys, nb, 256, 0, st, rt, m, h->d_keys_a.p, h->d_vals_a.p, h->d_flag.p);
+    CRANE_LAUNCH(k_rt_entry_keys, nb, 256, 0, st, rt, L.node_states(), h->work.d_keys_a.p, h->work.d_vals_a.p, h->d_flag.p);
     int bits = 8;
-    while ((1ull << bits) <= (uint64_t)h->n_slots) bits += 8;
+    while ((1ull << bits) <= (uint64_t)L.n_slots) bits += 8;
     TRY(radix_sort(h, E, bits, &keys, &vals));
-    CRANE_LAUNCH(k_rt_offsets, (h->n_slots + 1 + 255) / 256, 256, 0, st, keys, E, h->n_slots, h->d_rn_slot_off.p);
-    CRANE_LAUNCH(k_rt_slot_gather, (E + 255) / 256, 256, 0, st, rt, keys, vals, E, h->d_rn_slot_off.p + h->n_slots,
-                 h->d_rn_slot_end.p, h->d_rn_slot_res.p);
+    CRANE_LAUNCH(k_rt_offsets, (L.n_slots + 1 + 255) / 256, 256, 0, st, keys, E, L.n_slots, v.d_slot_off.p);
+    CRANE_LAUNCH(k_rt_slot_gather, (E + 255) / 256, 256, 0, st, rt, keys, vals, E, v.d_slot_off.p + L.n_slots,
+                 v.d_slot_end.p, v.d_slot_res.p);
   } else {
-    CU(cudaMemsetAsync(h->d_rn_slot_off.p, 0, sizeof(uint32_t) * ((size_t)h->n_slots + 1), st));
+    CU(cudaMemsetAsync(v.d_slot_off.p, 0, sizeof(uint32_t) * ((size_t)L.n_slots + 1), st));
   }
   // jobs by account: stable sort of the view's jobs by account
   if (R) {
-    CRANE_LAUNCH(k_rt_acc_keys, (R + 255) / 256, 256, 0, st, h->rn.d_rr_account.p, R, h->d_keys_a.p, h->d_vals_a.p);
+    CRANE_LAUNCH(k_rt_acc_keys, (R + 255) / 256, 256, 0, st, v.rn.d_rr_account.p, R, h->work.d_keys_a.p, h->work.d_vals_a.p);
     int bits = 8;
     while ((1ull << bits) <= (uint64_t)max_rn_account) bits += 8;
     TRY(radix_sort(h, R, bits, &keys, &vals));
-    CU(cudaMemcpyAsync(h->d_rn_acc_key.p, keys, sizeof(uint64_t) * R, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(h->d_rn_acc_job.p, vals, sizeof(uint32_t) * R, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(v.d_acc_key.p, keys, sizeof(uint64_t) * R, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(v.d_acc_job.p, vals, sizeof(uint32_t) * R, cudaMemcpyDeviceToDevice, st));
   }
   CU(cudaGetLastError());
   // a cluster with fewer nodes than the rows name: one flag read back
-  if (E && h->rr.node_bound > h->n_nodes) {
+  if (E && h->rr.node_bound > L.n_nodes) {
     uint32_t bad = 0;
     CU(cudaMemcpyAsync(&bad, h->d_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -1113,43 +1281,24 @@ int keep_running(crane_sched* h) {
   max_account = std::max(max_account, max_rn_account);
   const uint32_t A = (N + R) ? max_account + 1 : 0;
 
-  // ---- work + output buffers (the sorts of the regroup use the priority sort's) ----
-  size_t n1 = std::max<uint32_t>(N, 1);
-  const size_t ns = std::max<size_t>({n1, (size_t)Rt, (size_t)E});
-  CU(h->d_bounds.ensure(1));
-  CU(h->d_acc_service.ensure(std::max<uint32_t>(A, 1)));
-  CU(h->d_prio.ensure(n1));
-  CU(h->d_keys_a.ensure(ns));
-  CU(h->d_keys_b.ensure(ns));
-  CU(h->d_vals_a.ensure(ns));
-  CU(h->d_vals_b.ensure(ns));
-  uint32_t nq = std::min<uint32_t>(N, h->cfg.scheduled_batch_size);
-  CU(h->d_jobq.ensure(std::max<uint32_t>(nq, 1)));
-  CU(h->d_bitmap.ensure((size_t)std::max<uint32_t>(nq, 1) * h->words_per_row));
-  CU(h->d_reason.ensure(n1));
-  CU(h->d_out_prio.ensure(n1));
-  CU(h->d_out_start.ensure(n1));
-  CU(h->d_out_end.ensure(n1));
-  CU(h->d_out_nalloc.ensure(n1));
-  size_t ta = std::max<uint64_t>(h->pd.total_alloc, 1);
-  CU(h->d_out_node.ensure(ta));
-  CU(h->d_out_ntasks.ensure(ta));
-  CU(h->d_out_res.ensure(ta));
+  const uint32_t nq = std::min<uint32_t>(N, h->cfg.scheduled_batch_size);
+  CU(h->view.ensure(R, E, h->layout.n_slots, A));
+  CU(h->work.ensure(N, std::max<size_t>({(size_t)N, (size_t)Rt, (size_t)E}), A, nq, h->layout.words_per_row));
+  CU(h->outputs.ensure(N, h->pd.total_alloc));
 
   CU(cudaEventRecord(h->ev[kEvKeepBegin], st));
   if (h->rr.dirty) TRY(regroup(h, R, max_rn_account));
   // ---- accounts: offsets of the account groups, accounts present (pending included) ----
-  CU(h->d_rn_acc_off.ensure((size_t)A + 1));
-  CU(h->d_acc_present.ensure(std::max<uint32_t>(A, 1)));
-  CRANE_LAUNCH(k_rt_offsets, (A + 1 + 255) / 256, 256, 0, st, h->d_rn_acc_key.p, R, A, h->d_rn_acc_off.p);
-  CU(cudaMemsetAsync(h->d_acc_present.p, 0, std::max<uint32_t>(A, 1), st));
+  RunView& v = h->view;
+  CRANE_LAUNCH(k_rt_offsets, (A + 1 + 255) / 256, 256, 0, st, v.d_acc_key.p, R, A, v.d_acc_off.p);
+  CU(cudaMemsetAsync(v.d_acc_present.p, 0, std::max<uint32_t>(A, 1), st));
   if (N + R)
     CRANE_LAUNCH(k_acc_present, (N + R + 255) / 256, 256, 0, st, h->pd.d_account.p, h->pd.n_dead ? h->pd.d_dead.p : nullptr, N,
-                 h->rn.d_rr_account.p, R, h->d_acc_present.p);
+                 v.rn.d_rr_account.p, R, v.d_acc_present.p);
   CU(cudaEventRecord(h->ev[kEvKeepEnd], st));
   CU(cudaGetLastError());
-  h->n_running = R;
-  h->n_accounts = A;
+  v.n = R;
+  v.n_accounts = A;
   return CRANE_OK;
 }
 
@@ -1240,7 +1389,7 @@ int live_rows(crane_sched* h, const uint8_t* dead, uint32_t n, uint32_t n_live, 
   cudaStream_t st = h->stream;
   uint64_t* keys;
   uint32_t* vals;
-  CRANE_LAUNCH(k_rt_live_keys, (n + 255) / 256, 256, 0, st, dead, n, h->d_keys_a.p, h->d_vals_a.p);
+  CRANE_LAUNCH(k_rt_live_keys, (n + 255) / 256, 256, 0, st, dead, n, h->work.d_keys_a.p, h->work.d_vals_a.p);
   TRY(radix_sort(h, n, 8, &keys, &vals));
   if (n_live) CU(cudaMemcpyAsync(live, vals, sizeof(uint32_t) * n_live, cudaMemcpyDeviceToDevice, st));
   CU(cudaMemsetAsync(map, 0xff, sizeof(uint32_t) * n, st));
@@ -1373,7 +1522,7 @@ int check_step_jobs(crane_sched* h, const crane_step_jobs_t* jb) {
   if (jb->node_off[J] && (!jb->node || !jb->avail)) return fail(h, CRANE_EINVAL, "step jobs: null node table");
   for (uint32_t j = 0; j < J; ++j)
     for (uint32_t k = jb->node_off[j]; k < jb->node_off[j + 1]; ++k) {
-      if (jb->node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "step jobs[%u]: node %u out of range", j, jb->node[k]);
+      if (jb->node[k] >= h->layout.n_nodes) return fail(h, CRANE_EINVAL, "step jobs[%u]: node %u out of range", j, jb->node[k]);
       if (k > jb->node_off[j] && jb->node[k] <= jb->node[k - 1])
         return fail(h, CRANE_EINVAL, "step jobs[%u]: nodes must be ascending and distinct", j);
     }
@@ -1439,7 +1588,7 @@ int crane_sched_create(const crane_sched_config_t* cfg, int device, crane_sched_
     h->v2_budget = sm_total > stat + 1024 ? sm_total - stat - 1024 : 0;
     cudaFuncSetAttribute(k_commit2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->v2_budget);
   }
-  h->tl_cap = cfg->max_jobs_per_node + 1;
+  h->layout.tl_cap = cfg->max_jobs_per_node + 1;
   *out = h;
   return CRANE_OK;
 }
@@ -1459,25 +1608,24 @@ int crane_sched_set_cluster(crane_sched_t* h, const crane_cluster_t* c) {
   CU(cudaSetDevice(h->device));
   lower_stage(h, kNone);  // state of the previous cluster / tick is void from here on
   TRY(check_offsets(h, "cluster: part_off", c->part_off, c->n_partitions));
-  h->n_nodes = c->n_nodes;
-  h->n_parts = c->n_partitions;
-  memset(&h->dict, 0, sizeof h->dict);
-  h->dict.n_entries = c->n_gres_entries;
-  for (int e = 0; e < CRANE_GRES_ENTRIES; ++e) h->dict.entry_name[e] = c->gres_entry_name[e];
+  ClusterLayout& L = h->layout;
+  L.n_nodes = c->n_nodes;
+  L.n_parts = c->n_partitions;
+  memset(&L.dict, 0, sizeof L.dict);
+  L.dict.n_entries = c->n_gres_entries;
+  for (int e = 0; e < CRANE_GRES_ENTRIES; ++e) L.dict.entry_name[e] = c->gres_entry_name[e];
   for (uint32_t e = 0; e < c->n_gres_entries; ++e) {
     const uint8_t g = c->gres_entry_name[e];
-    if (h->dict.name_count[g] == 0) h->dict.name_first[g] = (uint8_t)e;
-    h->dict.name_count[g]++;
-    h->dict.name_mask8[g] |= 0xFFull << (8 * e);
+    if (L.dict.name_count[g] == 0) L.dict.name_first[g] = (uint8_t)e;
+    L.dict.name_count[g]++;
+    L.dict.name_mask8[g] |= 0xFFull << (8 * e);
   }
-  h->n_gres_entries = c->n_gres_entries;
-  h->c_res_total.assign(reinterpret_cast<const Row*>(c->res_total), reinterpret_cast<const Row*>(c->res_total) + c->n_nodes);
-  h->c_alive.assign(c->alive, c->alive + c->n_nodes);
-  h->c_drain.assign(c->drain, c->drain + c->n_nodes);
-  h->c_part_off.assign(c->part_off, c->part_off + c->n_partitions + 1);
-  h->c_part_nodes.assign(c->part_nodes, c->part_nodes + (c->n_partitions ? c->part_off[c->n_partitions] : 0));
-  h->r_start.clear(); h->r_end.clear(); h->r_node_off.assign(1, 0); h->r_node.clear(); h->r_res.clear();  // a new cluster has no reservations yet
-  h->n_resv = 0;
+  L.res_total.assign(reinterpret_cast<const Row*>(c->res_total), reinterpret_cast<const Row*>(c->res_total) + c->n_nodes);
+  L.alive.assign(c->alive, c->alive + c->n_nodes);
+  L.drain.assign(c->drain, c->drain + c->n_nodes);
+  L.part_off.assign(c->part_off, c->part_off + c->n_partitions + 1);
+  L.part_nodes.assign(c->part_nodes, c->part_nodes + (c->n_partitions ? c->part_off[c->n_partitions] : 0));
+  L.resv.reset();  // a new cluster has no reservations yet
   return build_layout(h);
 }
 
@@ -1492,28 +1640,27 @@ int crane_sched_set_reservations(crane_sched_t* h, const crane_reservations_t* r
     if (rv->end_time[r] < rv->start_time[r]) return fail(h, CRANE_EINVAL, "reservations[%u]: end before start", r);
     for (uint32_t k = rv->node_off[r]; k < rv->node_off[r + 1]; ++k) {
       if (!rv->node || !rv->res) return fail(h, CRANE_EINVAL, "reservations: null node table");
-      if (rv->node[k] >= h->n_nodes) return fail(h, CRANE_EINVAL, "reservations[%u]: node out of range", r);
+      if (rv->node[k] >= h->layout.n_nodes) return fail(h, CRANE_EINVAL, "reservations[%u]: node out of range", r);
       for (uint32_t k2 = rv->node_off[r]; k2 < k; ++k2)
         if (rv->node[k2] == rv->node[k]) return fail(h, CRANE_EINVAL, "reservations[%u]: node %u listed twice", r, rv->node[k]);
     }
   }
   lower_stage(h, kNone);
-  h->n_resv = n;
-  h->r_start.assign(rv ? rv->start_time : nullptr, rv ? rv->start_time + n : nullptr);
-  h->r_end.assign(rv ? rv->end_time : nullptr, rv ? rv->end_time + n : nullptr);
-  h->r_node_off.assign(1, 0);
-  h->r_node.clear();
-  h->r_res.clear();
+  Reservations& rs = h->layout.resv;
+  rs.reset();
+  rs.n = n;
+  rs.start.assign(rv ? rv->start_time : nullptr, rv ? rv->start_time + n : nullptr);
+  rs.end.assign(rv ? rv->end_time : nullptr, rv ? rv->end_time + n : nullptr);
   for (uint32_t r = 0; r < n; ++r) {
     // node states in node-index order: equal-cost nodes are ordered by index (deviation D1)
     std::vector<uint32_t> idx(rv->node_off[r + 1] - rv->node_off[r]);
     for (uint32_t k = 0; k < idx.size(); ++k) idx[k] = rv->node_off[r] + k;
     std::sort(idx.begin(), idx.end(), [&](uint32_t x, uint32_t y) { return rv->node[x] < rv->node[y]; });
     for (uint32_t k : idx) {
-      h->r_node.push_back(rv->node[k]);
-      h->r_res.push_back(reinterpret_cast<const Row&>(rv->res[k]));
+      rs.node.push_back(rv->node[k]);
+      rs.res.push_back(reinterpret_cast<const Row&>(rv->res[k]));
     }
-    h->r_node_off.push_back((uint32_t)h->r_node.size());
+    rs.node_off.push_back((uint32_t)rs.node.size());
   }
   return build_layout(h);
 }
@@ -1528,17 +1675,17 @@ int crane_sched_set_shard(crane_sched_t* h, uint32_t rank, uint32_t n_ranks, con
   h->h_part_owner.clear();
   h->h_part_list.clear();
   if (n_ranks > 1) {
-    if (!part_owner && h->n_parts) return fail(h, CRANE_EINVAL, "set_shard: null owner table");
-    std::vector<uint32_t> sched_owner(h->n_vparts, 0);  // reservations: rank 0
-    for (uint32_t p = 0; p < h->n_parts; ++p) {
+    if (!part_owner && h->layout.n_parts) return fail(h, CRANE_EINVAL, "set_shard: null owner table");
+    std::vector<uint32_t> sched_owner(h->layout.n_vparts, 0);  // reservations: rank 0
+    for (uint32_t p = 0; p < h->layout.n_parts; ++p) {
       if (part_owner[p] >= n_ranks) return fail(h, CRANE_EINVAL, "set_shard: partition %u owned by rank %u of %u", p, part_owner[p], n_ranks);
       h->h_part_owner.push_back(part_owner[p]);
-      const uint32_t c = h->h_part_comp[p];
-      if (h->h_part_cidx[p] == 0) sched_owner[c] = part_owner[p];
+      const uint32_t c = h->layout.h_part_comp[p];
+      if (h->layout.h_part_cidx[p] == 0) sched_owner[c] = part_owner[p];
       else if (sched_owner[c] != part_owner[p])
         return fail(h, CRANE_EINVAL, "set_shard: partitions that share nodes must have one owner (partition %u)", p);
     }
-    for (uint32_t c = 0; c < h->n_vparts; ++c)
+    for (uint32_t c = 0; c < h->layout.n_vparts; ++c)
       if (sched_owner[c] == rank) h->h_part_list.push_back(c);
     H2D(h->d_sched_owner, sched_owner.data(), sched_owner.size());
     H2D(h->d_part_owner, h->h_part_owner.data(), h->h_part_owner.size());
@@ -1551,13 +1698,14 @@ int crane_sched_set_shard(crane_sched_t* h, uint32_t rank, uint32_t n_ranks, con
 int crane_sched_device_placements(crane_sched_t* h, crane_device_placements_t* out) {
   if (!h || !out) return CRANE_EINVAL;
   TRY(require(h, kRan, "device_placements"));
-  out->reason = h->d_reason.p;
-  out->start_time = h->d_out_start.p;
-  out->end_time = h->d_out_end.p;
-  out->n_alloc = h->d_out_nalloc.p;
-  out->alloc_node = h->d_out_node.p;
-  out->alloc_ntasks = h->d_out_ntasks.p;
-  out->alloc_res = h->d_out_res.p;
+  const RunOutputs& o = h->outputs;
+  out->reason = o.d_reason.p;
+  out->start_time = o.d_start.p;
+  out->end_time = o.d_end.p;
+  out->n_alloc = o.d_nalloc.p;
+  out->alloc_node = o.d_node.p;
+  out->alloc_ntasks = o.d_ntasks.p;
+  out->alloc_res = o.d_res.p;
   out->n_jobs = h->pd.n;
   out->n_rows = h->pd.total_alloc;
   return CRANE_OK;
@@ -1634,7 +1782,7 @@ int crane_sched_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32
     H2D(h->d_start_rows, rows, n);
     CU(h->d_flag.ensure(1));
     CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
-    CRANE_LAUNCH(k_start_check, (n + 255) / 256, 256, 0, st, h->d_start_rows.p, n, h->d_reason.p, h->d_flag.p);
+    CRANE_LAUNCH(k_start_check, (n + 255) / 256, 256, 0, st, h->d_start_rows.p, n, h->outputs.d_reason.p, h->d_flag.p);
     uint32_t bad = 0;
     CU(cudaMemcpyAsync(&bad, h->d_flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -1653,13 +1801,8 @@ int crane_sched_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32
   H2D_AT(h->rr.d_rr_alloc_off, off.data(), base, (size_t)n + 1);
   std::vector<uint8_t> zeros(n, 0);
   H2D_AT(h->rr.d_dead, zeros.data(), base, n);
-  PlaceDev out{};
-  out.start_time = h->d_out_start.p;
-  out.end_time = h->d_out_end.p;
-  out.alloc_node = h->d_out_node.p;
-  out.alloc_res = h->d_out_res.p;
   const uint32_t nb = std::min<uint32_t>((n + 7) / 8, 8 * h->n_sm);
-  CRANE_LAUNCH(k_start, nb, 256, 0, st, h->pd.dev(), out, h->d_start_rows.p, n, base, h->rr.dev());
+  CRANE_LAUNCH(k_start, nb, 256, 0, st, h->pd.dev(), h->outputs.dev(), h->d_start_rows.p, n, base, h->rr.dev());
   // the pending rows leave the pending table (m_pending_job_map_.erase, JobScheduler.cpp:1305)
   CRANE_LAUNCH(k_mark_dead, (n + 255) / 256, 256, 0, st, h->d_start_rows.p, n, h->pd.d_dead.p);
   CU(cudaGetLastError());
@@ -1667,7 +1810,7 @@ int crane_sched_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32
     TRY(upload_call_rows(h, rows, n));
     DepEvents ev{};
     ev.mode = kFireStart;
-    ev.time = h->d_out_start.p;
+    ev.time = h->outputs.d_start.p;
     ev.base = base;
     TRY(dep_fire(h, ev, n, h->ent.n));
   }
@@ -1679,7 +1822,7 @@ int crane_sched_start(crane_sched_t* h, const uint32_t* rows, uint32_t n, uint32
   }
   h->pd.n_dead += n;
   h->rr.n = rows_end;
-  h->rr.node_bound = std::max(h->rr.node_bound, h->n_nodes);  // (placements are on this cluster's nodes)
+  h->rr.node_bound = std::max(h->rr.node_bound, h->layout.n_nodes);  // (placements are on this cluster's nodes)
   h->rr.dirty = true;
   CU(cudaStreamSynchronize(st));
   if (first_row) *first_row = base;
@@ -1825,11 +1968,7 @@ int crane_sched_compact(crane_sched_t* h, uint32_t* pending_map, uint32_t* runni
   const uint32_t Nl = N - h->pd.n_dead, Rl = Rt - h->rr.n_dead;
 
   // ---- work buffers, then the live rows, the maps and the open entries ----
-  const size_t ns = std::max<size_t>({(size_t)N, (size_t)Rt, (size_t)M, 1});
-  CU(h->d_keys_a.ensure(ns));
-  CU(h->d_keys_b.ensure(ns));
-  CU(h->d_vals_a.ensure(ns));
-  CU(h->d_vals_b.ensure(ns));
+  CU(h->work.ensure_sort(std::max<size_t>({(size_t)N, (size_t)Rt, (size_t)M})));
   CU(h->d_flag.ensure(1));
   DBuf<uint32_t> pd_live, pd_map, rr_live, rr_map, keep;
   if (cp_pd) {
@@ -1847,7 +1986,7 @@ int crane_sched_compact(crane_sched_t* h, uint32_t* pending_map, uint32_t* runni
     CU(keep.ensure(M));
     CU(cudaMemsetAsync(h->d_flag.p, 0, sizeof(uint32_t), st));
     CRANE_LAUNCH(k_cp_ent_keys, (M + 255) / 256, 256, 0, st, gate_dev(h), h->pd.dead(),
-                 h->d_keys_a.p, h->d_vals_a.p, h->d_flag.p);
+                 h->work.d_keys_a.p, h->work.d_vals_a.p, h->d_flag.p);
     uint64_t* keys;
     uint32_t* vals;
     TRY(radix_sort(h, M, 8, &keys, &vals));
@@ -1886,13 +2025,9 @@ int crane_sched_compact(crane_sched_t* h, uint32_t* pending_map, uint32_t* runni
   }
   if (cp_rr) std::swap(h->rr, rr);
   if (cp_ent) std::swap(h->ent, ent);
-  if (cp_pd || cp_rr) {
-    // work and output buffers sized for the old tables: keep_running sizes them again
-    h->d_keys_a.release(); h->d_keys_b.release(); h->d_vals_a.release(); h->d_vals_b.release();
-    h->d_prio.release(); h->d_g_code.release(); h->d_vpart.release(); h->d_jobq.release(); h->d_bitmap.release();
-    h->d_reason.release(); h->d_out_prio.release(); h->d_out_start.release(); h->d_out_end.release();
-    h->d_out_nalloc.release(); h->d_out_node.release(); h->d_out_ntasks.release(); h->d_out_res.release();
-    h->d_hist.release();
+  if (cp_pd || cp_rr) {  // (sized for the old tables)
+    h->work.release();
+    h->outputs.release();
   }
 
   // ---- the maps ----
@@ -1955,80 +2090,25 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
   lower_stage(h, kUploaded);  // the previous run's outputs are void from here on
   (void)cudaGetLastError();  // a stale error of an earlier, unrelated call in this process is not this run's
   cudaStream_t st = h->stream;
-  const uint32_t N = h->pd.n, R = h->n_running;
+  const ClusterLayout& L = h->layout;
+  RunWork& w = h->work;
+  const uint32_t N = h->pd.n, R = h->view.n, A = h->view.n_accounts;
   h->timing.kernel_launches = 0;
-
   PendingDev pd = h->pd.dev();
-
-  RunningDev rn{};
-  rn.n = R;
-  rn.start_time = h->rn.d_rr_start.p;
-  rn.end_time = h->rn.d_rr_end.p;
-  rn.node_num = h->rn.d_rr_node_num.p;
-  rn.partition_priority = h->rn.d_rr_part_prio.p;
-  rn.qos_priority = h->rn.d_rr_qos_prio.p;
-  rn.account = h->rn.d_rr_account.p;
-  rn.view_cpu_raw = h->rn.d_rr_cpu.p;
-  rn.view_mem = h->rn.d_rr_mem.p;
-  rn.slot_off = h->d_rn_slot_off.p;
-  rn.slot_end = h->d_rn_slot_end.p;
-  rn.slot_res = h->d_rn_slot_res.p;
-  rn.n_accounts = h->n_accounts;
-  rn.acc_off = h->d_rn_acc_off.p;
-  rn.acc_job = h->d_rn_acc_job.p;
-  rn.acc_present = h->d_acc_present.p;
-
-  ClusterDev cl{};
-  cl.n_slots = h->n_slots;
-  cl.n_parts = h->n_parts;
-  cl.n_vparts = h->n_vparts;
-  cl.n_comp = h->n_comp;
-  cl.part_comp = h->d_part_comp.p;
-  cl.part_cidx = h->d_part_cidx.p;
-  cl.slot_memb = h->max_comp_parts > 1 ? h->d_slot_memb.p : nullptr;
-  cl.n_resv = h->n_resv;
-  cl.resv_start = h->d_resv_start.p;
-  cl.resv_end = h->d_resv_end.p;
-  cl.slot_resv = h->d_slot_resv.p;
-  cl.rsv_off = h->d_rsv_off.p;
-  cl.rsv_id = h->d_rsv_id.p;
-  cl.rsv_res = h->d_rsv_res.p;
-  cl.max_part_slots = h->max_part_slots;
-  cl.part_base = h->d_part_base.p;
-  cl.slot_node = h->d_slot_node.p;
-  cl.node_slot = h->d_node_slot.p;
-  cl.slot_total = h->d_slot_total.p;
-  cl.slot_class = h->d_slot_class.p;
-  cl.class_rows = h->d_class_rows.p;
-
-  TimelineDev tl{};
-  tl.cap = h->tl_cap;
-  tl.n = h->d_tl_n.p;
-  tl.ent = h->d_tl_ent.p;
-  tl.avail0 = h->d_avail0.p;
-  tl.cost0 = h->d_cost0.p;
-  tl.skip = h->d_skip.p;
-  tl.first_resv = h->d_first_resv.p;
-
-  PlaceDev out{};
-  out.reason = h->d_reason.p;
-  out.priority = h->d_out_prio.p;
-  out.start_time = h->d_out_start.p;
-  out.end_time = h->d_out_end.p;
-  out.n_alloc = h->d_out_nalloc.p;
-  out.alloc_node = h->d_out_node.p;
-  out.alloc_ntasks = h->d_out_ntasks.p;
-  out.alloc_res = h->d_out_res.p;
+  const RunningDev rn = h->view.dev();
+  const ClusterDev cl = L.dev();
+  const TimelineDev tl = L.timelines();
+  const PlaceDev out = h->outputs.dev();
 
   // ---- node state / timelines (R2,R3,R4) -----------------------------------
   CU(cudaEventRecord(h->ev[kEvRunBegin], st));
   if (h->pd.total_alloc) {  // allocation slots of jobs without a placement read as zero
-    CU(cudaMemsetAsync(h->d_out_node.p, 0, sizeof(uint32_t) * h->pd.total_alloc, st));
-    CU(cudaMemsetAsync(h->d_out_ntasks.p, 0, sizeof(uint32_t) * h->pd.total_alloc, st));
-    CU(cudaMemsetAsync(h->d_out_res.p, 0, sizeof(Row) * h->pd.total_alloc, st));
+    CU(cudaMemsetAsync(out.alloc_node, 0, sizeof(uint32_t) * h->pd.total_alloc, st));
+    CU(cudaMemsetAsync(out.alloc_ntasks, 0, sizeof(uint32_t) * h->pd.total_alloc, st));
+    CU(cudaMemsetAsync(out.alloc_res, 0, sizeof(Row) * h->pd.total_alloc, st));
   }
-  if (h->n_slots) {
-    CRANE_LAUNCH(k_node_init, (h->n_slots + 127) / 128, 128, 0, st, cl, rn, tl, now, h->cfg.max_jobs_per_node, h->cfg.cost_policy);
+  if (L.n_slots) {
+    CRANE_LAUNCH(k_node_init, (L.n_slots + 127) / 128, 128, 0, st, cl, rn, tl, now, h->cfg.max_jobs_per_node, h->cfg.cost_policy);
     h->timing.kernel_launches++;
   }
   CU(cudaEventRecord(h->ev[kEvInitEnd], st));
@@ -2037,23 +2117,23 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
   const bool gated = h->gate.on && N;
   if (gated) {
     TRY(gate_fit(h));
-    CU(h->d_g_code.ensure(N));
-    CRANE_LAUNCH(k_gate, (N + 255) / 256, 256, 0, st, gate_dev(h), now, h->d_g_code.p);
-    pd.dead = h->d_g_code.p;
+    CU(w.d_g_code.ensure(N));
+    CRANE_LAUNCH(k_gate, (N + 255) / 256, 256, 0, st, gate_dev(h), now, w.d_g_code.p);
+    pd.dead = w.d_g_code.p;
     h->timing.kernel_launches++;
     // an account with only gated rows does not seed the fair-share bounds
-    if (h->n_accounts) {
-      CU(cudaMemsetAsync(h->d_acc_present.p, 0, h->n_accounts, st));
-      CRANE_LAUNCH(k_acc_present, (N + R + 255) / 256, 256, 0, st, h->pd.d_account.p, h->d_g_code.p, N,
-                   h->rn.d_rr_account.p, R, h->d_acc_present.p);
+    if (A) {
+      CU(cudaMemsetAsync(h->view.d_acc_present.p, 0, A, st));
+      CRANE_LAUNCH(k_acc_present, (N + R + 255) / 256, 256, 0, st, h->pd.d_account.p, w.d_g_code.p, N,
+                   rn.account, R, h->view.d_acc_present.p);
       h->timing.kernel_launches++;
     }
   }
 
   // ---- priority + queue (R5,R6) --------------------------------------------
   uint32_t nq_cap = std::min<uint32_t>(N, h->cfg.scheduled_batch_size);
-  CU(cudaMemsetAsync(h->d_part_count.p, 0, sizeof(uint32_t) * (h->n_vparts + 2), st));
-  CU(h->d_vpart.ensure(std::max<uint32_t>(N, 1)));
+  CU(cudaMemsetAsync(L.d_part_count.p, 0, sizeof(uint32_t) * (L.n_vparts + 2), st));
+  CU(w.d_vpart.ensure(std::max<uint32_t>(N, 1)));
   if (N) {
     PrioCfg pc{};
     pc.type = h->cfg.priority_type;
@@ -2064,80 +2144,78 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     pc.w_part = h->cfg.weight_partition;
     pc.w_qos = h->cfg.weight_qos;
     pc.max_age = h->cfg.max_age_s;
-    uint64_t* keys = h->d_keys_a.p;
-    uint32_t* vals = h->d_vals_a.p;
+    uint64_t* keys = w.d_keys_a.p;
+    uint32_t* vals = w.d_vals_a.p;
     if (pc.type != 0) {
-      CRANE_LAUNCH(k_bounds_init, 1, 32, 0, st, h->d_bounds.p);
+      CRANE_LAUNCH(k_bounds_init, 1, 32, 0, st, w.d_bounds.p);
       uint32_t nb = std::min<uint32_t>((N + R + 255) / 256, 4 * h->n_sm);
-      CRANE_LAUNCH(k_bounds, nb, 256, 0, st, pd, rn, now, (uint64_t)h->cfg.max_age_s, h->d_bounds.p);
+      CRANE_LAUNCH(k_bounds, nb, 256, 0, st, pd, rn, now, (uint64_t)h->cfg.max_age_s, w.d_bounds.p);
       h->timing.kernel_launches += 2;
-      if (h->n_accounts) {
-        CU(cudaMemsetAsync(h->d_acc_service.p, 0, sizeof(double) * h->n_accounts, st));
-        CRANE_LAUNCH(k_service, (h->n_accounts + 127) / 128, 128, 0, st, rn, now, h->d_bounds.p, h->d_acc_service.p);
+      if (A) {
+        CU(cudaMemsetAsync(w.d_acc_service.p, 0, sizeof(double) * A, st));
+        CRANE_LAUNCH(k_service, (A + 127) / 128, 128, 0, st, rn, now, w.d_bounds.p, w.d_acc_service.p);
         h->timing.kernel_launches++;
       }
     }
-    CRANE_LAUNCH(k_priority, (N + 255) / 256, 256, 0, st, pd, pc, now, h->d_bounds.p, h->d_acc_service.p,
-                 h->d_prio.p, h->d_keys_a.p, h->d_vals_a.p);
+    CRANE_LAUNCH(k_priority, (N + 255) / 256, 256, 0, st, pd, pc, now, w.d_bounds.p, w.d_acc_service.p,
+                 w.d_prio.p, w.d_keys_a.p, w.d_vals_a.p);
     h->timing.kernel_launches++;
     if (pc.type != 0 || h->pd.n_dead || gated)  // (FIFO keeps input order; excluded rows only have to go behind the others)
       TRY(radix_sort(h, N, pc.type != 0 ? 64 : 8, &keys, &vals));
     // keys2 go to the buffer not holding `vals`
-    uint64_t* key2 = h->d_keys_a.p;
+    uint64_t* key2 = w.d_keys_a.p;
     uint32_t* order = vals;
-    if (order != h->d_vals_a.p) {
+    if (order != w.d_vals_a.p) {
       // radix_sort works on the (keys_a, vals_a) pair: bring the order back
-      CU(cudaMemcpyAsync(h->d_vals_a.p, order, sizeof(uint32_t) * N, cudaMemcpyDeviceToDevice, st));
-      order = h->d_vals_a.p;
+      CU(cudaMemcpyAsync(w.d_vals_a.p, order, sizeof(uint32_t) * N, cudaMemcpyDeviceToDevice, st));
+      order = w.d_vals_a.p;
     }
-    CRANE_LAUNCH(k_queue_keys, (N + 255) / 256, 256, 0, st, pd, order, h->d_prio.p, h->cfg.scheduled_batch_size,
-                 cl, now, key2, out, h->d_part_count.p, h->d_vpart.p);
-    CRANE_LAUNCH(k_part_offsets, 1, 32, 0, st, h->d_part_count.p, h->n_vparts, h->d_part_job_off.p);
+    CRANE_LAUNCH(k_queue_keys, (N + 255) / 256, 256, 0, st, pd, order, w.d_prio.p, h->cfg.scheduled_batch_size,
+                 cl, now, key2, out, L.d_part_count.p, w.d_vpart.p);
+    CRANE_LAUNCH(k_part_offsets, 1, 32, 0, st, L.d_part_count.p, L.n_vparts, L.d_part_job_off.p);
     h->timing.kernel_launches += 2;
     int bits = 8;
-    while ((1ull << bits) < (uint64_t)h->n_vparts + 2) bits += 8;
+    while ((1ull << bits) < (uint64_t)L.n_vparts + 2) bits += 8;
     uint64_t* k2s;
     uint32_t* queue;
     TRY(radix_sort(h, N, bits, &k2s, &queue));
-    h->d_queue = queue;
     if (nq_cap) {
       // n_queued <= nq_cap lives on the device (part_job_off[n_parts]); the
       // kernels below bound themselves with it.
-      CRANE_LAUNCH(k_build_jobq, (nq_cap + 127) / 128, 128, 0, st, pd, queue, h->d_part_job_off.p + h->n_vparts, h->d_jobq.p, (uint32_t)h->dict_slot, h->d_vpart.p, h->n_comp, h->d_part_cidx.p);
+      CRANE_LAUNCH(k_build_jobq, (nq_cap + 127) / 128, 128, 0, st, pd, queue, L.d_part_job_off.p + L.n_vparts, w.d_jobq.p, (uint32_t)h->dict_slot, w.d_vpart.p, L.n_comp, L.d_part_cidx.p);
       h->timing.kernel_launches++;
     }
   } else {
-    CRANE_LAUNCH(k_part_offsets, 1, 32, 0, st, h->d_part_count.p, h->n_vparts, h->d_part_job_off.p);
+    CRANE_LAUNCH(k_part_offsets, 1, 32, 0, st, L.d_part_count.p, L.n_vparts, L.d_part_job_off.p);
     h->timing.kernel_launches++;
   }
   CU(cudaEventRecord(h->ev[kEvPrioEnd], st));
 
   // ---- capability bitmap (R7 predicate + R8) -------------------------------
-  if (nq_cap && h->n_vparts) {
+  if (nq_cap && L.n_vparts) {
     uint32_t wpb = 8;
     uint32_t nb = std::min<uint32_t>((nq_cap + wpb - 1) / wpb, 8 * h->n_sm);
-    CRANE_LAUNCH(k_feas_bitmap, nb, wpb * 32, 0, st, cl, pd, h->d_jobq.p, h->d_part_job_off.p + h->n_vparts, h->words_per_row, h->d_bitmap.p,
+    CRANE_LAUNCH(k_feas_bitmap, nb, wpb * 32, 0, st, cl, pd, w.d_jobq.p, L.d_part_job_off.p + L.n_vparts, L.words_per_row, w.d_bitmap.p,
                  h->shard_n > 1 ? h->d_sched_owner.p : nullptr, h->shard_rank, (uint32_t)h->dict_slot);
     h->timing.kernel_launches++;
   }
   CU(cudaEventRecord(h->ev[kEvFeasEnd], st));
 
   // ---- sequential commit (R7,R9,R10,R11) -----------------------------------
-  if (nq_cap && h->n_vparts) {
+  if (nq_cap && L.n_vparts) {
     Commit2Args c2{};
-    c2.cl = cl; c2.tl = tl; c2.jobq = h->d_jobq.p; c2.part_job_off = h->d_part_job_off.p; c2.bitmap = h->d_bitmap.p;
-    c2.words_per_row = h->words_per_row; c2.ring = h->v2_ring; c2.out = out; c2.now = now;
+    c2.cl = cl; c2.tl = tl; c2.jobq = w.d_jobq.p; c2.part_job_off = L.d_part_job_off.p; c2.bitmap = w.d_bitmap.p;
+    c2.words_per_row = L.words_per_row; c2.ring = L.v2_ring; c2.out = out; c2.now = now;
     c2.max_window = h->cfg.max_time_window_s; c2.max_jobs = h->cfg.max_jobs_per_node; c2.cost_policy = h->cfg.cost_policy;
-    CU(h->d_prof.ensure((size_t)h->n_vparts * 16));
-    c2.prof = h->d_prof.p;
-    c2.gres = h->dict.n_entries > 0 ? 1u : 0u;
-    c2.sched_nparts = h->max_comp_parts > 1 ? h->d_sched_nparts.p : nullptr;
-    c2.slot_memb = h->d_slot_memb.p;
+    c2.prof = L.d_prof.p;
+    c2.gres = L.dict.n_entries > 0 ? 1u : 0u;
+    c2.sched_nparts = L.max_comp_parts > 1 ? L.d_sched_nparts.p : nullptr;
+    c2.slot_memb = L.d_slot_memb.p;
     c2.dslot = (uint32_t)h->dict_slot;
     c2.req_node = h->pd.d_req_node.p;
     c2.req_task = h->pd.d_req_task.p;
-    size_t smem = commit2_smem_bytes(h->max_part_slots, h->words_per_row, c2.gres != 0, h->v2_ring, h->max_comp_parts);
-    uint32_t grid = h->n_vparts;
+    size_t smem = commit2_smem_bytes(L.max_part_slots, L.words_per_row, c2.gres != 0, L.v2_ring, L.max_comp_parts);
+    uint32_t grid = L.n_vparts;
     if (h->shard_n > 1) {
       c2.part_list = h->d_part_list.p;
       grid = (uint32_t)h->h_part_list.size();
@@ -2145,7 +2223,7 @@ int crane_sched_run(crane_sched_t* h, int64_t now) {
     if (grid) CRANE_LAUNCH(k_commit2, grid, kT2, smem, st, c2);
     h->timing.kernel_launches++;
     if (h->shard_n > 1 && N) {
-      CRANE_LAUNCH(k_shard_mask, (N + 255) / 256, 256, 0, st, pd, out, h->d_part_owner.p, h->n_parts, h->shard_rank);
+      CRANE_LAUNCH(k_shard_mask, (N + 255) / 256, 256, 0, st, pd, out, h->d_part_owner.p, L.n_parts, h->shard_rank);
       h->timing.kernel_launches++;
     }
   }
@@ -2165,18 +2243,19 @@ int crane_sched_fetch(crane_sched_t* h, crane_placements_t* out) {
     return fail(h, CRANE_EINVAL, "placements: null column");
   if (h->pd.total_alloc && (!out->alloc_node || !out->alloc_ntasks || !out->alloc_res))
     return fail(h, CRANE_EINVAL, "placements: null allocation table");
+  const RunOutputs& o = h->outputs;
   // slots of jobs without a placement stay zero
   if (N) {
-    CU(cudaMemcpyAsync(out->reason, h->d_reason.p, N, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(out->priority, h->d_out_prio.p, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(out->start_time, h->d_out_start.p, sizeof(int64_t) * N, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(out->end_time, h->d_out_end.p, sizeof(int64_t) * N, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(out->n_alloc, h->d_out_nalloc.p, sizeof(uint32_t) * N, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->reason, o.d_reason.p, N, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->priority, o.d_prio.p, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->start_time, o.d_start.p, sizeof(int64_t) * N, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->end_time, o.d_end.p, sizeof(int64_t) * N, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->n_alloc, o.d_nalloc.p, sizeof(uint32_t) * N, cudaMemcpyDeviceToHost, st));
   }
   if (h->pd.total_alloc) {
-    CU(cudaMemcpyAsync(out->alloc_node, h->d_out_node.p, sizeof(uint32_t) * h->pd.total_alloc, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(out->alloc_ntasks, h->d_out_ntasks.p, sizeof(uint32_t) * h->pd.total_alloc, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(out->alloc_res, h->d_out_res.p, sizeof(Row) * h->pd.total_alloc, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->alloc_node, o.d_node.p, sizeof(uint32_t) * h->pd.total_alloc, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->alloc_ntasks, o.d_ntasks.p, sizeof(uint32_t) * h->pd.total_alloc, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->alloc_res, o.d_res.p, sizeof(Row) * h->pd.total_alloc, cudaMemcpyDeviceToHost, st));
   }
   memcpy(out->alloc_off, h->pd.h_alloc_off.data(), sizeof(uint32_t) * ((size_t)N + 1));
   CU(cudaEventRecord(h->ev[kEvD2hEnd], st));
@@ -2210,9 +2289,9 @@ int crane_sched_debug_profile(crane_sched_t* h, unsigned long long* dst, size_t 
   if (!h || !dst) return CRANE_EINVAL;
   TRY(require(h, kRan, "debug_profile"));
   CU(cudaSetDevice(h->device));
-  size_t n = std::min(cap, (size_t)h->n_vparts * 16);
+  size_t n = std::min(cap, (size_t)h->layout.n_vparts * 16);
   CU(cudaStreamSynchronize(h->stream));
-  if (n) CU(cudaMemcpy(dst, h->d_prof.p, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  if (n) CU(cudaMemcpy(dst, h->layout.d_prof.p, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   return CRANE_OK;
 }
 
@@ -2276,15 +2355,15 @@ int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_
   q.chain_off = h->d_q_chain_off.p; q.chain_acct = h->d_q_chain.p;
   q.user_usage = h->d_q_user_usage.p; q.account_usage = h->d_q_acct_usage.p; q.qos_usage = h->d_q_qos_usage.p;
   q.qos = h->pd.d_qos.p; q.user = h->pd.d_user.p; q.time_limit = h->pd.d_time_limit.p;
-  q.n_alloc = h->d_out_nalloc.p; q.alloc_off = h->pd.d_alloc_off.p; q.alloc_res = h->d_out_res.p;
-  q.reason = h->d_reason.p;
+  q.n_alloc = h->outputs.d_nalloc.p; q.alloc_off = h->pd.d_alloc_off.p; q.alloc_res = h->outputs.d_res.p;
+  q.reason = h->outputs.d_reason.p;
   if (N) {
     // the jobs the pass walks, grouped by qos in job-id order: key + stable radix sort
     const int bits = Q < 255 ? 8 : 16;
     const uint64_t sentinel = (1ull << bits) - 1;
     CU(cudaEventRecord(h->ev[kEvQosBegin], h->stream));
-    CU(h->d_keys_a.ensure(N)); CU(h->d_keys_b.ensure(N)); CU(h->d_vals_a.ensure(N)); CU(h->d_vals_b.ensure(N));
-    CRANE_LAUNCH(k_qos_keys, (N + 255) / 256, 256, 0, h->stream, q, h->d_keys_a.p, h->d_vals_a.p, sentinel);
+    CU(h->work.ensure_sort(N));
+    CRANE_LAUNCH(k_qos_keys, (N + 255) / 256, 256, 0, h->stream, q, h->work.d_keys_a.p, h->work.d_vals_a.p, sentinel);
     uint64_t* keys;
     uint32_t* list;
     TRY(radix_sort(h, N, bits, &keys, &list));
@@ -2296,12 +2375,12 @@ int crane_sched_qos_filter(crane_sched_t* h, const crane_qos_table_t* qt, uint8_
     const uint32_t in_smem = !force_global && table_bytes + 40 * 1024 <= h->v2_budget ? 1u : 0u;
     const size_t dyn = in_smem ? table_bytes : 0;
     CU(cudaFuncSetAttribute(k_qos_chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-    CRANE_LAUNCH(k_qos_chain, Q, kQosThreads, dyn, h->stream, q, h->dict, list, h->d_q_off.p, in_smem);
+    CRANE_LAUNCH(k_qos_chain, Q, kQosThreads, dyn, h->stream, q, h->layout.dict, list, h->d_q_off.p, in_smem);
     CU(cudaGetLastError());
     CU(cudaEventRecord(h->ev[kEvQosEnd], h->stream));
     h->timing.kernel_launches += 3;
   }
-  if (N) CU(cudaMemcpyAsync(reason, h->d_reason.p, N, cudaMemcpyDeviceToHost, h->stream));
+  if (N) CU(cudaMemcpyAsync(reason, h->outputs.d_reason.p, N, cudaMemcpyDeviceToHost, h->stream));
   if ((size_t)U * Q) CU(cudaMemcpyAsync(qt->user_usage, h->d_q_user_usage.p, (size_t)U * Q * sizeof(crane_meta_resource_t), cudaMemcpyDeviceToHost, h->stream));
   if ((size_t)A * Q) CU(cudaMemcpyAsync(qt->account_usage, h->d_q_acct_usage.p, (size_t)A * Q * sizeof(crane_meta_resource_t), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaMemcpyAsync(qt->qos_usage, h->d_q_qos_usage.p, (size_t)Q * sizeof(crane_meta_resource_t), cudaMemcpyDeviceToHost, h->stream));
@@ -2771,11 +2850,11 @@ int crane_sched_debug_bitmap(crane_sched_t* h, uint32_t* dst, size_t cap_words, 
   TRY(require(h, kRan, "debug_bitmap"));
   CU(cudaSetDevice(h->device));
   uint32_t nq = 0;
-  CU(cudaMemcpy(&nq, h->d_part_job_off.p + h->n_vparts, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(&nq, h->layout.d_part_job_off.p + h->layout.n_vparts, sizeof(uint32_t), cudaMemcpyDeviceToHost));
   if (rows) *rows = nq;
-  if (words_per_row) *words_per_row = h->words_per_row;
-  size_t n = std::min(cap_words, (size_t)nq * h->words_per_row);
-  if (dst && n) CU(cudaMemcpy(dst, h->d_bitmap.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  if (words_per_row) *words_per_row = h->layout.words_per_row;
+  size_t n = std::min(cap_words, (size_t)nq * h->layout.words_per_row);
+  if (dst && n) CU(cudaMemcpy(dst, h->work.d_bitmap.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   return CRANE_OK;
 }
 
