@@ -14,6 +14,9 @@
 // Live rows and kept entries keep their order, so every order-sensitive step of a run
 // (the stable priority sort, FIFO, the regroup's sorts and fp64 sums, account grouping)
 // sees the same sequence as on the uncompacted tables.
+// crane_sched_steps_compact rewrites the resident step tables with the same gathers (the
+// host lists their live rows, since it holds every flag that decides liveness) and
+// k_cp_spans for the allocation pool.
 #pragma once
 
 #include "sched_kernels.cuh"
@@ -86,6 +89,25 @@ __global__ void k_cp_csr(const uint32_t* off, const T* src, const uint32_t* live
   for (uint32_t c = blockIdx.x * warps + warp_id(); c < n_live; c += gridDim.x * warps) {
     const uint32_t r = live[c], s0 = off[r], n = off[r + 1] - s0, d0 = new_off[c];
     for (uint32_t k = lane; k < n; k += 32) dst[d0 + k] = src[s0 + k];
+  }
+}
+
+// crane_sched_steps_compact: one warp per kept scheduled step (old row rows[c], new row
+// new_rows[c]); its node_num node rows of the allocation pool move from alloc_at[old] to
+// new_at[c], and lane 0 points the new alloc_at there. A step's span is not a CSR row (the
+// spans lie in the order the passes scheduled them, not in row order), hence not k_cp_csr.
+__global__ void k_cp_spans(const uint32_t* alloc_at, const uint32_t* node_num, const uint32_t* sa_node,
+                           const Row* sa_res, const uint32_t* rows, const uint32_t* new_rows, const uint32_t* new_at,
+                           uint32_t n, uint32_t* new_alloc_at, uint32_t* new_sa_node, Row* new_sa_res) {
+  const int lane = lane_id();
+  const uint32_t warps = blockDim.x >> 5;
+  for (uint32_t c = blockIdx.x * warps + warp_id(); c < n; c += gridDim.x * warps) {
+    const uint32_t r = rows[c], s0 = alloc_at[r], cnt = node_num[r], d0 = new_at[c];
+    for (uint32_t k = lane; k < cnt; k += 32) {
+      new_sa_node[d0 + k] = sa_node[s0 + k];
+      new_sa_res[d0 + k] = sa_res[s0 + k];
+    }
+    if (lane == 0) new_alloc_at[new_rows[c]] = d0;
   }
 }
 

@@ -356,6 +356,10 @@ struct StepJobTable {
   DBuf<uint32_t> d_node_off, d_node;
   DBuf<Row> d_avail;
 
+  // no fixed-width columns: a job is its CSR rows (d_node_off, d_node, d_avail)
+  template <class F>
+  void each(StepJobTable&, F) {}
+
   void mark_dirty(uint32_t j) {
     if (!h_dirty[j]) {
       h_dirty[j] = 1;
@@ -397,6 +401,19 @@ struct StepTable {
   DBuf<View> d_req_node, d_req_task;
   DBuf<uint32_t> d_sa_node;
   DBuf<Row> d_sa_res;
+
+  // (the list CSRs d_incl_off / d_incl, d_excl_off / d_excl and the allocation pool are not here)
+  template <class F>
+  void each(StepTable& o, F f) {
+    f(d_job, o.d_job);
+    f(d_nn, o.d_nn);
+    f(d_nt, o.d_nt);
+    f(d_t0, o.d_t0);
+    f(d_t1, o.d_t1);
+    f(d_req_node, o.d_req_node);
+    f(d_req_task, o.d_req_task);
+    f(d_alloc_at, o.d_alloc_at);
+  }
 
   void reset() {
     n = n_alloc = 0;
@@ -1538,6 +1555,107 @@ void launch_steps(crane_sched* h, const StepJobsDev& dj, const StepsDev& ds, con
 // grid of a kernel with one warp per item, 256 threads per block
 uint32_t warp_grid(const crane_sched* h, uint64_t items) {
   return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((items + 7) / 8, 8ull * h->n_sm));
+}
+
+// What crane_sched_steps_compact keeps, decided on the host from its mirrors: a step-job
+// row unless step_jobs_erase erased it; a step row unless it was erased or its job was
+// (such a step is still pending or scheduled in h_state). Kept rows keep their order.
+struct StepsKept {
+  std::vector<uint8_t> jdead, sdead;  // [old rows] the row goes
+  std::vector<uint32_t> jmap, smap;   // [old rows] its new row, or kRowNone
+  uint32_t Jl = 0, Sl = 0, K = 0, A = 0;  // kept jobs, steps, scheduled steps, allocation rows
+  // uploaded: live jobs [Jl] | live steps [Sl] | their new job rows [Sl] | the kept scheduled steps [K],
+  // their new rows [K], their new allocation offsets [K] (the exclusive scan of node_num over them)
+  std::vector<uint32_t> u;
+
+  StepsKept(const StepJobTable& sj, const StepTable& sp)
+      : jdead(sj.h_dead), sdead(sp.n), jmap(sj.n, kRowNone), smap(sp.n, kRowNone) {
+    std::vector<uint32_t> sched, sched_new, sched_at, job;
+    for (uint32_t j = 0; j < sj.n; ++j)
+      if (!jdead[j]) {
+        jmap[j] = Jl++;
+        u.push_back(j);
+      }
+    for (uint32_t s = 0; s < sp.n; ++s) {
+      sdead[s] = sp.h_state[s] == kSpErased || jdead[sp.h_job[s]];
+      if (sdead[s]) continue;
+      if (sp.h_state[s] == kSpScheduled) {
+        sched.push_back(s);
+        sched_new.push_back(Sl);
+        sched_at.push_back(A);
+        A += sp.h_nn[s];
+      }
+      job.push_back(jmap[sp.h_job[s]]);
+      smap[s] = Sl++;
+      u.push_back(s);
+    }
+    K = (uint32_t)sched.size();
+    for (const auto* v : {&job, &sched, &sched_new, &sched_at}) u.insert(u.end(), v->begin(), v->end());
+  }
+};
+
+// The compacted step tables: the host state of the kept rows of the handle's, the device
+// buffers allocated for steps_copy
+int steps_fresh(crane_sched* h, const StepsKept& kp, StepJobTable& sj, StepTable& sp) {
+  const StepJobTable& oj = h->sj;
+  const StepTable& os = h->sp;
+  sj.n = kp.Jl;
+  sj.h_node_off = live_offsets(oj.h_node_off, kp.jdead);
+  sj.h_dead.assign(kp.Jl, 0);
+  sj.h_dirty = live_only(oj.h_dirty, kp.jdead);
+  for (uint32_t j : oj.h_dirty_rows)  // (old rows)
+    if (!kp.jdead[j]) sj.h_dirty_rows.push_back(kp.jmap[j]);
+  for (uint32_t j = 0; j < oj.n; ++j) {
+    if (kp.jdead[j]) continue;
+    sj.h_queue.emplace_back();
+    for (uint32_t s : oj.h_queue[j]) sj.h_queue.back().push_back(kp.smap[s]);
+  }
+  sp.n = kp.Sl;
+  sp.n_alloc = kp.A;
+  sp.h_job.assign(kp.u.begin() + kp.Jl + kp.Sl, kp.u.begin() + kp.Jl + 2 * (size_t)kp.Sl);
+  sp.h_nn = live_only(os.h_nn, kp.sdead);
+  sp.h_nt = live_only(os.h_nt, kp.sdead);
+  sp.h_state = live_only(os.h_state, kp.sdead);
+  sp.h_incl_off = live_offsets(os.h_incl_off, kp.sdead);
+  sp.h_excl_off = live_offsets(os.h_excl_off, kp.sdead);
+  const size_t j1 = std::max<uint32_t>(kp.Jl, 1), s1 = std::max<uint32_t>(kp.Sl, 1);
+  CU(ensure_cols(sj, kp.Jl));
+  CU(sj.d_node_off.ensure(j1 + 1));
+  CU(sj.d_node.ensure(std::max<uint32_t>(sj.h_node_off.back(), 1)));
+  CU(sj.d_avail.ensure(std::max<uint32_t>(sj.h_node_off.back(), 1)));
+  CU(ensure_cols(sp, kp.Sl));
+  CU(sp.d_incl_off.ensure(s1 + 1));
+  CU(sp.d_excl_off.ensure(s1 + 1));
+  CU(sp.d_incl.ensure(std::max<uint32_t>(sp.h_incl_off.back(), 1)));
+  CU(sp.d_excl.ensure(std::max<uint32_t>(sp.h_excl_off.back(), 1)));
+  CU(sp.d_sa_node.ensure(std::max<uint32_t>(kp.A, 1)));
+  CU(sp.d_sa_res.ensure(std::max<uint32_t>(kp.A, 1)));
+  return CRANE_OK;
+}
+
+// The kept rows of the handle's step tables into the fresh ones; du = the uploaded StepsKept::u
+int steps_copy(crane_sched* h, const StepsKept& kp, StepJobTable& sj, StepTable& sp, const uint32_t* du) {
+  StepJobTable& oj = h->sj;
+  StepTable& os = h->sp;
+  const uint32_t Jl = kp.Jl, Sl = kp.Sl, K = kp.K;
+  const uint32_t* jl = du, *sl = du + Jl, *job = sl + Sl, *sched = job + Sl;
+  ColSet cs{};
+  oj.each(sj, gather_to(cs, Jl));
+  os.each(sp, gather_to(cs, Sl));
+  TRY(gather(h, cs, sl, Sl));
+  // the job column through the job map
+  if (Sl) CU(cudaMemcpyAsync(sp.d_job.p, job, sizeof(uint32_t) * Sl, cudaMemcpyDeviceToDevice, h->stream));
+  TRY(csr_offsets(h, oj.d_node_off.p, jl, Jl, sj.d_node_off.p));
+  TRY(csr_copy(h, oj.d_node_off.p, oj.d_node.p, jl, Jl, sj.d_node_off.p, sj.d_node.p));
+  TRY(csr_copy(h, oj.d_node_off.p, oj.d_avail.p, jl, Jl, sj.d_node_off.p, sj.d_avail.p));
+  TRY(csr_offsets(h, os.d_incl_off.p, sl, Sl, sp.d_incl_off.p));
+  TRY(csr_copy(h, os.d_incl_off.p, os.d_incl.p, sl, Sl, sp.d_incl_off.p, sp.d_incl.p));
+  TRY(csr_offsets(h, os.d_excl_off.p, sl, Sl, sp.d_excl_off.p));
+  TRY(csr_copy(h, os.d_excl_off.p, os.d_excl.p, sl, Sl, sp.d_excl_off.p, sp.d_excl.p));
+  if (K)
+    CRANE_LAUNCH(k_cp_spans, warp_grid(h, K), 256, 0, h->stream, os.d_alloc_at.p, os.d_nn.p, os.d_sa_node.p,
+                 os.d_sa_res.p, sched, sched + K, sched + 2 * K, K, sp.d_alloc_at.p, sp.d_sa_node.p, sp.d_sa_res.p);
+  return CRANE_OK;
 }
 
 }  // namespace
@@ -2835,6 +2953,41 @@ int crane_sched_step_jobs_avail(crane_sched_t* h, const uint32_t* rows, uint32_t
   CU(cudaMemcpyAsync(dst, h->d_steps_rows.p, (size_t)E * sizeof(Row), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
   CU(cudaGetLastError());
+  return CRANE_OK;
+}
+
+int crane_sched_step_rows(const crane_sched_t* h, uint32_t* step_jobs, uint32_t* steps, uint32_t* alloc_rows) {
+  if (!h) return CRANE_EINVAL;
+  if (step_jobs) *step_jobs = h->sj.n;
+  if (steps) *steps = h->sp.n;
+  if (alloc_rows) *alloc_rows = h->sp.n_alloc;
+  return CRANE_OK;
+}
+
+int crane_sched_steps_compact(crane_sched_t* h, uint32_t* step_job_map, uint32_t* step_map) {
+  if (!h) return CRANE_EINVAL;
+  TRY(require(h, kCluster, "steps_compact"));
+  CU(cudaSetDevice(h->device));
+  h->sr.valid = false;
+  cudaStream_t st = h->stream;
+  const StepsKept kp(h->sj, h->sp);
+  const uint32_t J = h->sj.n, S = h->sp.n;
+  if (kp.Jl < J || kp.Sl < S) {
+    // ---- every new buffer before the first gather: CRANE_ENOMEM leaves the tables as they were ----
+    StepJobTable sj;
+    StepTable sp;
+    TRY(steps_fresh(h, kp, sj, sp));
+    H2D(h->d_sp_call, kp.u.data(), kp.u.size());
+    // ---- gathers, then the new tables replace the old ones (whose buffers go with the locals) ----
+    TRY(steps_copy(h, kp, sj, sp, h->d_sp_call.p));
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(st));
+    std::swap(h->sj, sj);
+    std::swap(h->sp, sp);
+  }
+  // (identity maps when nothing was erased)
+  if (step_job_map) std::copy(kp.jmap.begin(), kp.jmap.end(), step_job_map);
+  if (step_map) std::copy(kp.smap.begin(), kp.smap.end(), step_map);
   return CRANE_OK;
 }
 

@@ -1,7 +1,8 @@
 // step_resident_kernels.cuh — sm_90a kernels of the device-resident step state of running
 // jobs (JobInCtld::step_res_avail_ and pending_step_ids_, CtldPublicDefs.h:984-1009).
 //
-// Two resident tables whose rows keep their index until crane_sched_step_jobs_reset:
+// Two resident tables whose rows keep their index until crane_sched_steps_compact
+// (compact_kernels.cuh) or crane_sched_step_jobs_reset:
 //   step jobs  one row per running job that can get steps: its nodes (ascending) and one
 //              step_res_avail_ row per node, in a node pool (CSR sj_node_off);
 //   steps      one row per step: its crane_steps_t columns, and once scheduled the offset

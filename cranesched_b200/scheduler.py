@@ -122,6 +122,10 @@ def load_library(path: str | None = None) -> C.CDLL:
     lib.crane_sched_step_jobs_reset.argtypes = [C.c_void_p]
     lib.crane_sched_compact.restype = C.c_int
     lib.crane_sched_compact.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.crane_sched_step_rows.restype = C.c_int
+    lib.crane_sched_step_rows.argtypes = [C.c_void_p, P(C.c_uint32), P(C.c_uint32), P(C.c_uint32)]
+    lib.crane_sched_steps_compact.restype = C.c_int
+    lib.crane_sched_steps_compact.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     _libs[path] = lib
     return lib
 
@@ -137,7 +141,7 @@ EXPORTS = ("crane_sched_create", "crane_sched_destroy", "crane_sched_last_error"
            "crane_sched_running_end", "crane_sched_step_jobs_start", "crane_sched_step_jobs_append",
            "crane_sched_step_jobs_erase", "crane_sched_steps_append", "crane_sched_steps_erase", "crane_sched_steps_run",
            "crane_sched_steps_fetch", "crane_sched_step_jobs_avail", "crane_sched_step_jobs_reset",
-           "crane_sched_compact")
+           "crane_sched_compact", "crane_sched_step_rows", "crane_sched_steps_compact")
 
 
 class GpuScheduler:
@@ -387,6 +391,24 @@ class GpuScheduler:
 
     def step_jobs_reset(self):
         self._check(self._lib.crane_sched_step_jobs_reset(self._h))
+
+    def step_rows(self) -> tuple[int, int, int]:
+        """(step jobs, steps, allocation-pool rows) of the resident step tables, tombstones included."""
+        j, s, a = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
+        self._check(self._lib.crane_sched_step_rows(self._h, C.byref(j), C.byref(s), C.byref(a)))
+        return j.value, s.value, a.value
+
+    def steps_compact(self, maps: bool = True) -> tuple[np.ndarray | None, np.ndarray | None]:
+        """Drops the erased step jobs, the erased steps and the steps of erased jobs, and
+        the allocation rows of the steps that go, on the device; running steps keep their
+        allocation. Returns (step_job_map, step_map): uint32, the new row of every old row
+        or abi.ROW_NONE (None, None when `maps` is false: the call then passes NULL maps)."""
+        j, s, _ = self.step_rows()
+        jm = np.zeros(j, np.uint32) if maps else None
+        sm = np.zeros(s, np.uint32) if maps else None
+        self._check(self._lib.crane_sched_steps_compact(self._h, None if jm is None else jm.ctypes.data,
+                                                        None if sm is None else sm.ctypes.data))
+        return jm, sm
 
     def timing(self) -> dict:
         t = abi.TimingC()

@@ -616,8 +616,9 @@ int crane_sched_schedule_steps(crane_sched_t* h, const crane_step_jobs_t* jobs,
 /* The daemon's step state changes by small events; these calls keep it on the device
  * across passes of the step scheduler thread (JobScheduler.cpp:1637-1665) instead of
  * re-sending every job with pending steps to crane_sched_schedule_steps on every pass.
- * Two tables whose rows keep their index until crane_sched_step_jobs_reset (which is
- * also how a caller compacts their tombstones: reset, then re-append the live rows):
+ * Two tables whose rows keep their index until crane_sched_steps_compact drops their
+ * erased rows in place (running steps' allocations included), or until
+ * crane_sched_step_jobs_reset empties them (how a caller starts over):
  *   step jobs  one row per running job that can get steps: its nodes (ascending and
  *              distinct) and one step_res_avail_ row per node. Independent of the running
  *              table: set_running, running_erase / running_end, set_cluster and every
@@ -692,6 +693,30 @@ int crane_sched_steps_fetch(crane_sched_t* h, crane_step_results_t* out);
 int crane_sched_step_jobs_avail(crane_sched_t* h, const uint32_t* rows, uint32_t n, crane_res_in_node_t* dst,
                                 uint32_t* n_node_rows);
 int crane_sched_step_jobs_reset(crane_sched_t* h);
+/* Rows of the resident step tables, tombstones included (any pointer may be NULL): step
+ * jobs, steps, and node rows of the allocation pool. */
+int crane_sched_step_rows(const crane_sched_t* h, uint32_t* step_jobs, uint32_t* steps, uint32_t* alloc_rows);
+/* Compaction of the step tables. Erased rows stay behind in both tables, and every
+ * scheduled step's node rows stay in the allocation pool even after it ends, so the
+ * tables only grow. crane_sched_steps_compact rewrites them on the device, keeping only
+ * what is live:
+ *   step jobs  rows erased by step_jobs_erase go. step_job_map[old] (step_jobs of
+ *              step_rows before the call) = the new row, or CRANE_ROW_NONE. A kept job
+ *              keeps its nodes and avail rows byte for byte, its dirty flag and its queue.
+ *   steps      erased steps and every step of an erased job go; pending and scheduled
+ *              steps stay in their state. step_map[old] likewise.
+ *   pool       only the node rows of the scheduled steps that stay, each step pointing at
+ *              its new span: a later steps_erase of it gives the same rows back.
+ * Kept rows keep their relative order (the new index is the rank among kept rows), so a
+ * job's FIFO queue, later appends and every pass's results are unchanged at the mapped
+ * rows. Either map may be NULL; with nothing erased the tables stay as they are and the
+ * maps are the identity. Needs set_cluster, voids the last steps_fetch as every step call
+ * does, and leaves NodeSelect alone (crane_sched_compact and this call touch disjoint
+ * tables). Every new buffer is allocated before the first copy, so CRANE_ENOMEM leaves the
+ * tables as they were; afterwards device memory holds the kept rows plus the usual
+ * headroom. Only row indices cross PCIe, host to device. When to compact is the caller's
+ * choice. */
+int crane_sched_steps_compact(crane_sched_t* h, uint32_t* step_job_map, uint32_t* step_map);
 
 /* Capability bitmap of the last run (the jobs x nodes feasibility bitmap):
  * bit (rank r, local node q) set iff the r-th job in priority order can run
